@@ -6,7 +6,7 @@
     python bench.py --impl reference ...                      (the reference's CPU path = oracle port, host cores)
 
 One "step" = one ``PruningHarness.train_step`` call over one batch (the product's own step, not a copy of it):
-H2D (e2e only) -> zero_grad -> autocast forward through the sm_100a masked-conv kernels -> CE loss -> backward
+H2D (e2e only) -> zero_grad -> autocast forward through the sm_90a masked-conv kernels -> CE loss -> backward
 (dgrad/wgrad kernels, mask fused in wgrad) -> P2P gradient mean over NVLink under the backward pass (N>1) -> fused SGD
 -> LR scheduler step.  Nothing is skipped in the timed region.
 
@@ -30,15 +30,32 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 METRIC = "images_per_sec_resnet50_erk80_train_step"
 GFLOP_PER_IMG = 24.30           # SURVEY.md §8(d): fwd 8.178 + dgrad 7.942 + wgrad 8.178 (masked layers, dense)
-ROOFLINE_IMG_S = 39.8e3         # SURVEY.md §8(d): per-layer max(tensor, HBM) masked-GEMM roofline per GPU
+DUMP_SAMPLE = 1 << 20           # --dump-outputs: parameters sampled after the last timed step (4 MiB of float32)
+DUMP_SEED = 1234
+
+
+def dump_outputs(path, loss, model):
+    """What the last timed ``train_step`` produced: its loss, and a fixed seeded sample of the parameters it updated
+    (concatenated in ``model.parameters()`` order), as float32 .npy files."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+    np.save(os.path.join(path, "loss.npy"), loss.detach().float().cpu().numpy().astype(np.float32))
+    with torch.no_grad():
+        flat = torch.cat([p.detach().float().flatten() for p in model.parameters()])
+    g = torch.Generator().manual_seed(DUMP_SEED)
+    idx = torch.randperm(flat.numel(), generator=g)[:DUMP_SAMPLE].sort().values
+    np.save(os.path.join(path, "params_sample.npy"), flat[idx.to(flat.device)].cpu().numpy().astype(np.float32))
 
 
 def peaks():
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.isfile(path):
         d = json.load(open(path))
-        return dict(hbm=d["hbm_gbs"], tf=d["bf16_tflops_sustained"], tf_burst=d["bf16_tflops"], src="measured")
-    return dict(hbm=6650.0, tf=1400.0, tf_burst=1590.0, src="fallback")
+        return dict(hbm=d["hbm_gbs"], tf=d["bf16_tflops_sustained"], tf_burst=d["bf16_tflops"],
+                    src_hbm="measured HBM copy bandwidth", src_tf="measured sustained bf16")
+    return dict(hbm=3350.0, tf=989.0, tf_burst=989.0,
+                src_hbm="H100 SXM data sheet HBM3 bandwidth (not measured)", src_tf="H100 SXM data sheet dense bf16 (not measured)")
 
 
 class ClockSampler:
@@ -189,7 +206,7 @@ def run_reference(args):
 
 
 def gpu_eager_reference(dev, B, steps, world):
-    """The kernels to beat (BASELINE.md §5): the reference's own GPU execution model — cuDNN convs on mask*w, ATen
+    """The kernels to beat: the reference's own GPU execution model — cuDNN convs on mask*w, ATen
     BatchNorm / ReLU, torch.optim.SGD under bf16 autocast (the oracle's module graph moved to cuda), ATen kthvalue on
     the concatenated scores (pruning_utils.py:75-79), NCCL all_reduce of the 102 MB gradient (world > 1)."""
     import torch
@@ -276,6 +293,8 @@ def main():
     ap.add_argument("--no-graph", action="store_true", help="do not capture the train step into a CUDA graph")
     ap.add_argument("--no-overlap", action="store_true", help="launch the gradient exchange after the backward pass")
     ap.add_argument("--no-wgrad-side-stream", action="store_true", help="keep the weight-gradient GEMMs on the compute stream")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's loss and a seeded sample of the updated parameters as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -360,9 +379,14 @@ def main():
     # ---- device-resident run (value) ----
     clocks = ClockSampler(local_rank); clocks.start()
 
+    last = {}
+
     def dev_step(i):
-        loss_acc.add_(step(next(batches)))
+        last["loss"] = step(next(batches))
+        loss_acc.add_(last["loss"])
     ms_total = timed(K, dev_step)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["loss"], model)
     launches = launches_per_step * K
     clk = clocks.stop()
     if harness.reducer is not None:
@@ -401,21 +425,24 @@ def main():
         h.remove()
     first = next(iter(io))
     per_img = sum(3 * (a + b) for a, b in io.values()) - sum(io[first])          # elements per 2 images
+    # per-layer roofline of the masked GEMMs (dense FLOPs): each op takes at least max(FLOPs / tensor peak, bytes / HBM peak)
+    wdims = {name: (m.weight.shape[0], m.weight.numel()) for name, m in model._masked()}
+    t_tensor = t_hbm = t_roof = 0.0                                                # seconds per image
+    for name, (a, b) in io.items():
+        nops = 2 if name == first else 3                                           # the stem has no dgrad
+        f = nops * 2.0 * b * (wdims[name][1] / wdims[name][0]) / 2
+        by = nops * 2.0 * (a + b) / 2
+        t_tensor += f / (pk["tf"] * 1e12); t_hbm += by / (pk["hbm"] * 1e9)
+        t_roof += max(f / (pk["tf"] * 1e12), by / (pk["hbm"] * 1e9))
+    roofline_img_s = 1.0 / t_roof
     alg_bytes_step = 2.0 * per_img / 2 * B
     achieved_gbs = alg_bytes_step * K / (gemm_ms / 1e3) / 1e9 if gemm_ms > 0 else 0.0
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "r02_igemm_traffic.json")
-    if not os.path.isfile(tpath):
-        tpath = os.path.join(ROOT, "profiles", "r01_igemm_traffic.json")
-    if os.path.isfile(tpath) and B == 512:
-        traffic = json.load(open(tpath))["dram_bytes_per_launch"]
     n_launch = sum(v[2] for v in tot.values()) / KT
     roofline = {"bound": "hbm", "achieved": achieved_gbs, "peak": pk["hbm"], "unit": "GB/s",
-                "frac": achieved_gbs / pk["hbm"], "traffic": traffic,
-                "traffic_note": f"dram read+write per igemm kernel launch, ncu over one eager step at B=512 ({os.path.relpath(tpath, ROOT)})" if traffic else None,
-                "peak_source": pk["src"] + " HBM copy bandwidth",
-                "kernel": "k_igemm_fwd (fprop+dgrad) / k_igemm_wgrad — masked implicit GEMM, tcgen05 + TMA",
-                "why_hbm": "sum over the 54 layers: conv I/O bytes / HBM peak (11.4 ms at B=512) exceeds FLOPs / tensor peak (8.5 ms); 30 of 54 layers are HBM-bound",
+                "frac": achieved_gbs / pk["hbm"], "traffic": None,
+                "peak_source": pk["src_hbm"],
+                "kernel": "k_igemm_fwd (fprop+dgrad) / k_igemm_wgrad — masked implicit GEMM, wgmma + TMA",
+                "why_hbm": f"sum over the masked layers at B={B}: conv I/O bytes / HBM peak {t_hbm * B * 1e3:.1f} ms, FLOPs / tensor peak {t_tensor * B * 1e3:.1f} ms",
                 "algorithmic_bytes_per_step": alg_bytes_step, "algorithmic_bytes_per_launch": alg_bytes_step / n_launch,
                 "launches_per_step": n_launch,
                 "timing": f"CUDA events around each masked-GEMM C-ABI call over {KT} eager harness.train_step calls ({ms_eager / KT:.2f} ms/step eager); step rate from the harness's CUDA-graph replay" if use_graph else "CUDA events, eager",
@@ -423,8 +450,9 @@ def main():
                 "by_op_ms_per_step": {k: v[0] / KT for k, v in tot.items()},
                 "share_of_step": gemm_ms / ms_total,
                 "tensor": {"achieved_tflops": achieved_tf, "peak_tflops": pk["tf"], "frac": achieved_tf / pk["tf"],
-                           "flops_per_step": GFLOP_PER_IMG * 1e9 * B, "peak_source": pk["src"] + " sustained bf16"},
-                "frac_of_masked_gemm_roofline_img_s": (img_s / world) / ROOFLINE_IMG_S}
+                           "flops_per_step": GFLOP_PER_IMG * 1e9 * B, "peak_source": pk["src_tf"]},
+                "masked_gemm_roofline_img_s": roofline_img_s,
+                "frac_of_masked_gemm_roofline_img_s": (img_s / world) / roofline_img_s}
 
     # ---- end-to-end run: pinned host batches -> DevicePrefetcher (copy stream, double-buffered) -> harness.train_step,
     # ---- loss read back every step like the reference's loss.item() (base_harness.py:134) ----
@@ -462,7 +490,7 @@ def main():
             other = torch.zeros(64 * 1024 * 1024, dtype=torch.float32, device=dev) if clean else None
             tms, info = [], None
             for _ in range(reps):
-                flush.zero_()                                  # 256 MiB write: evicts the 126 MB L2
+                flush.zero_()                                  # 256 MiB write: evicts the 50 MB L2
                 if clean:                                      # ... and leaves it full of DIRTY lines whose write-back competes with the
                     other.sum()                                # timed kernel for DRAM; reading another 256 MiB leaves clean, unrelated lines
                 a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -534,7 +562,7 @@ def main():
                        "global_batch": B * world, "per_gpu_batch": B, "parallelism": f"dp{world}",
                        "api": "PruningHarness.train_step (conf_b200/synthetic_rn50_erk80.yaml)",
                        "inputs": "fresh Philox batch generated on the device every step (generation inside the timed region)",
-                       "sparsity_percent": sparsity, "cuda_graph": bool(use_graph), "l2": "inputs (308 MB/batch at B=512) and activations exceed the 126 MB L2",
+                       "sparsity_percent": sparsity, "cuda_graph": bool(use_graph), "l2": "inputs (308 MB/batch at B=512) and activations exceed the 50 MB L2",
                        "grad_exchange": "none (1 GPU)" if world == 1 else
                        ("tp_p2p_allreduce over symmetric memory (NVLink), per-bucket on a side stream under the backward pass, mask applied in the kernel; no NCCL on the data path"
                         + ("" if not args.no_overlap else " [overlap disabled]"))},

@@ -1,5 +1,5 @@
 /*
- * turboprune_b200 — C ABI of the B200-native (sm_100a) TurboPrune hot path.
+ * turboprune_b200 — C ABI of the H100-native (sm_90a) TurboPrune hot path.
  *
  * Plain C types only: device pointers as void*, sizes as int64_t / size_t, the CUDA
  * stream as an opaque void* (a cudaStream_t / CUstream; NULL = default stream).  No
@@ -30,7 +30,7 @@ extern "C" {
 #define TP_ERR_CUDA          -3   /* a CUDA runtime/driver call failed (see tp_last_cuda_error) */
 #define TP_ERR_K_RANGE       -4   /* k out of [1, N] — torch.kthvalue raises for this (k == 0!) */
 #define TP_ERR_UNSUPPORTED   -5   /* valid request this build does not implement */
-#define TP_ERR_DEVICE        -6   /* not an sm_100 device */
+#define TP_ERR_DEVICE        -6   /* not an sm_90 device */
 
 const char* tp_strerror(int code);
 const char* tp_last_cuda_error(void);      /* text of the last CUDA error seen by this thread */
@@ -170,10 +170,10 @@ int tp_cifar_augment(const void* src, void* out, const int64_t* shifts, const ui
 int tp_synth_normal(void* out, int64_t numel, uint64_t seed, uint64_t counter_offset, int raw_words, void* stream);
 int tp_synth_labels(void* out, int64_t numel, int num_classes, uint64_t seed, uint64_t counter_offset, void* stream);
 
-/* ---- masked implicit-GEMM convolution / linear on tcgen05 tensor cores -----------------
+/* ---- masked implicit-GEMM convolution / linear on wgmma tensor cores -------------------
  * Replaces F.conv2d / F.linear / F.conv1d(k=1) on the masked weight
  * (utils/mask_layers.py:26-34, :70, :110-118) and their autograd backward.
- * Activations are NHWC bf16 (channels_last), accumulation fp32 in TMEM.
+ * Activations are NHWC bf16 (channels_last), accumulation fp32.
  *
  * tp_conv_desc describes one convolution; linear layers are 1x1 convs with H = W = 1.
  */

@@ -9,11 +9,10 @@ baseline.  The product path (``turboprune_b200``) never imports it and fails lou
 when the CUDA library is missing.
 
 Pinning: the reference ships no tests, golden vectors or fixtures (SURVEY.md §4), so
-parity is pinned by outputs of the reference itself executed in the build container:
-``tests/golden/make_golden.py`` imports the unmodified reference modules from
-``/root/reference`` and writes the fixtures under ``tests/golden/``;
-``tests/test_oracle_golden.py`` checks every oracle function against them (and, when
-``/root/reference`` is present, against the live reference).
+parity is pinned by outputs of the reference itself: ``tests/golden/make_golden.py`` and
+``tests/golden/make_reference_golden.py`` import the unmodified reference modules from a
+checkout of it and write the fixtures under ``tests/golden/``; ``tests/test_oracle_golden.py``
+checks every oracle function against them.
 """
 from .mask_ops import (  # noqa: F401
     masked_conv2d, masked_linear, masked_conv1d_k1,

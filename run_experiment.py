@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Level loop — drop-in for the reference's ``run_experiment.py`` (:21-133) on the B200 hot path.
+"""Level loop — drop-in for the reference's ``run_experiment.py`` (:21-133) on the H100 hot path.
 
     python run_experiment.py --config-name=cifar10_er_erk [--config-path=/path/to/TurboPrune/conf] group.key=value ...
     torchrun --nproc_per_node=N run_experiment.py --config-name=imagenet_er_balanced ...

@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""Reference-style GPU eager path vs this repo's path on the same box (SURVEY.md §8(d), last row).
+"""Reference-style GPU eager path vs this repo's path on the same GPU (SURVEY.md §8(d), last row).
 
-The reference is a GPU framework: on a B200 it would run the masked layers as ``F.conv2d(x, mask * w)`` on
+The reference is a GPU framework: on an H100 it would run the masked layers as ``F.conv2d(x, mask * w)`` on
 cuDNN under bf16 autocast, torchvision BatchNorm/ReLU, ``torch.optim.SGD`` (mask_layers.py:26-34,
-base_harness.py:115-134).  /root/reference does not travel to the GPU box, so the oracle's restatement of that
-module graph (oracle/model.py — the same torch ops, validated against the real reference in tests/) is moved to
+base_harness.py:115-134).  The reference is not part of this repository, so the oracle's restatement of that
+module graph (oracle/model.py — the same torch ops, validated against the reference's recorded outputs in tests/) is moved to
 ``cuda`` and timed here: this is the "kernel to beat".  It lives under tests/ because it executes oracle/ code;
 it is a script (not collected by pytest):
 
@@ -104,7 +104,7 @@ def main():
         loss_t = my_step()
     ms_graph = timed(gr.replay, steps)
     print(json.dumps({
-        "workload": f"resnet50 ERK-80 train step, B={B}, bf16 autocast, SGD(0.9, 1e-4), 1x B200",
+        "workload": f"resnet50 ERK-80 train step, B={B}, bf16 autocast, SGD(0.9, 1e-4), 1x {torch.cuda.get_device_name()}",
         "reference_style_eager_cudnn": {"ms_per_step": ms_ref, "img_s": B / ms_ref * 1e3, "loss_after": loss_ref},
         "this_repo_eager": {"ms_per_step": ms_eager, "img_s": B / ms_eager * 1e3},
         "this_repo_cuda_graph": {"ms_per_step": ms_graph, "img_s": B / ms_graph * 1e3, "loss_last": float(loss_t)},

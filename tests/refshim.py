@@ -1,14 +1,15 @@
-"""Import the UNMODIFIED reference (/root/reference) inside the build container.
+"""Import the UNMODIFIED reference (a checkout at $TURBOPRUNE_REFERENCE) for fixture generation.
 
 Test/fixture infrastructure only.  The reference needs a handful of packages that
-are not in this image (fastargs, omegaconf, timm, ...); we inject empty stand-ins
+are not installed here (fastargs, omegaconf, timm, ...); we inject empty stand-ins
 for them into ``sys.modules`` so that ``utils.mask_layers``,
 ``utils.pruning_utils`` and ``utils.custom_models`` import unchanged.
 
-``/root/reference`` does not exist on the GPU box, so nothing under ``-m gpu``,
-``bench.py`` or ``smoke()`` may call :func:`load_reference`; it is used by
-``tests/golden/make_golden.py`` (fixture generation) and by the CPU tests that
-cross-check ``oracle/`` against the real reference when it is present.
+Only the two fixture generators, ``tests/golden/make_golden.py`` and
+``tests/golden/make_reference_golden.py``, call :func:`load_reference` /
+:func:`load_reference_dataset`; no test imports the reference itself — the tests
+compare against the fixtures those scripts wrote under ``tests/golden/``.
+``make_cfg`` and ``make_harness`` are used by the tests.
 """
 import importlib
 import os

@@ -150,29 +150,26 @@ def test_allreduce_mean_mask_fixed_order():
     assert np.array_equal(out, ref.astype(np.float32))
 
 
-def test_oracle_matches_live_reference_when_present():
-    import refshim
-    if not refshim.reference_available():
-        pytest.skip("/root/reference not mounted (GPU box)")
-    ml, pu, cm = refshim.load_reference()
+def test_oracle_matches_reference_model_and_prune():
+    """oracle.model / oracle.prune against the reference's own ResNet-18 (construction, eval forward, prune_mag), as
+    recorded from it by tests/golden/make_reference_golden.py."""
+    import hashlib
     import oracle.model as om
-    torch.manual_seed(0); ref = cm.TorchVisionModel(refshim.make_cfg("resnet18", "cifar10"))
+    z = np.load(os.path.join(G, "reference_live.npz"))
     torch.manual_seed(0); mine = om.build("resnet18", "cifar10")
-    for (k1, a), (k2, b) in zip(ref.model.state_dict().items(), mine.state_dict().items()):
-        assert k1 == k2 and torch.equal(a, b)
-    x = torch.randn(4, 3, 32, 32)
-    ref.eval(); mine.eval()
-    assert torch.equal(ref(x), mine(x))
+    ref_sha = dict(zip(z["sd_sha256.keys"].tolist(), z["sd_sha256.values"].tolist()))
+    for k, v in mine.state_dict().items():
+        assert hashlib.sha256(v.detach().contiguous().numpy().tobytes()).hexdigest() == ref_sha[f"init.model.{k}"], k
+    mine.eval()
+    with torch.no_grad():
+        assert np.array_equal(mine(torch.from_numpy(z["rn18.x"])).numpy(), z["rn18.logits"])
     layers = om.masked_layers(mine)
     new, thr, k = P.prune_global([m.weight.detach().numpy() for _, m in layers], [m.mask.numpy() for _, m in layers], 0.8)
-    pu.prune_mag(ref, 0.8)
-    rm = [m.mask.numpy() for m in ref.model.modules() if isinstance(m, (ml.ConvMask, ml.Conv1dMask, ml.LinearMask))]
-    assert all(np.array_equal(a, b) for a, b in zip(new, rm))
-    h = json.load(open(os.path.join(G, "imp_hashes.json")))
-    import hashlib
     hh = hashlib.sha256()
     for a in new:
         hh.update(np.ascontiguousarray(a).tobytes())
+    assert hh.hexdigest() == str(z["rn18.mag08.masks_sha256"])
+    h = json.load(open(os.path.join(G, "imp_hashes.json")))
     assert hh.hexdigest() == h["levels"][0]["masks_sha256"]
     assert int(np.float32(thr).view(np.uint32)) == h["levels"][0]["thr_bits"]
 
@@ -180,7 +177,7 @@ def test_oracle_matches_live_reference_when_present():
 # ---------------------------------------------------------------- data path (SURVEY §8(f) row 3) --------------------
 def test_augmentation_oracle_matches_reference_fixture_and_live():
     """oracle.data.batch_crop / batch_flip_lr / batch_cutout / augment against outputs of the reference's own functions
-    (utils/dataset.py:38-98, fixture written by make_golden.py) and, when /root/reference is mounted, against a live run."""
+    (utils/dataset.py:38-98, fixtures written by make_golden.py and make_reference_golden.py)."""
     from oracle import data as D
     z = np.load(os.path.join(G, "aug_small.npz"))
     assert np.array_equal(D.batch_crop(z["padded"], 12, z["crop2.shifts"]), z["crop2.out"])
@@ -188,15 +185,10 @@ def test_augmentation_oracle_matches_reference_fixture_and_live():
     assert np.array_equal(D.batch_flip_lr(z["imgs"], z["flip.mask"]), z["flip.out"])
     assert np.array_equal(D.batch_cutout(z["imgs"], 5, z["cut.y"], z["cut.x"]), z["cut.out"])
     assert np.array_equal(D.augment(z["padded4"], 12, z["epoch.shifts"], z["epoch.mask"], 3, z["epoch.y"], z["epoch.x"]), z["epoch.out"])
-    import refshim
-    if refshim.reference_available():
-        ds = refshim.load_reference_dataset()
-        g = torch.Generator().manual_seed(3)
-        imgs = torch.randn(5, 3, 10, 10, generator=g)
-        pad = torch.nn.functional.pad(imgs, (3,) * 4, "reflect")
-        torch.manual_seed(8); ref = ds.batch_crop(pad, 10)
-        torch.manual_seed(8); sh = torch.randint(-3, 4, size=(5, 2))
-        assert np.array_equal(D.batch_crop(pad.numpy(), 10, sh.numpy()), ref.numpy())
+    r = np.load(os.path.join(G, "reference_live.npz"))
+    torch.manual_seed(8); sh = torch.randint(-3, 4, size=(5, 2))          # the draw batch_crop makes under this seed
+    assert np.array_equal(sh.numpy(), r["crop.shifts"])
+    assert np.array_equal(D.batch_crop(r["crop.pad"], 10, r["crop.shifts"]), r["crop.out"])
 
 
 def test_philox_known_answer_and_generator_statistics():

@@ -99,7 +99,7 @@ def config4():
 
 
 def config5():
-    """1 process: per-GPU batch 64 on one GPU.  Under torchrun: data parallel over all ranks (BASELINE.json: 8 x B200), SNIP
+    """1 process: per-GPU batch 64 on one GPU.  Under torchrun: data parallel over all ranks (BASELINE.json config 5), SNIP
     scored on every rank's first batch, rank 0's masks imposed, gradient exchange over NVLink under the backward pass."""
     import refshim
     from turboprune_b200.utils import custom_models as cm, pruning_utils as pu

@@ -7,6 +7,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import torch
 from turboprune_b200 import ops, _cabi
+from bench import peaks
 
 LAYERS = [  # name, cin, cout, k, stride, pad, hw_in, count
     ("l1.1x1 64->64", 64, 64, 1, 1, 0, 56, 1), ("l1.1x1 256->64", 256, 64, 1, 1, 0, 56, 2), ("l1.3x3 64", 64, 64, 3, 1, 1, 56, 3),
@@ -32,9 +33,9 @@ def main():
         ops.set_kblock_skip(False)
     B = int(sys.argv[1]) if len(sys.argv) > 1 else 256
     only = sys.argv[2] if len(sys.argv) > 2 else None
-    pk = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.isfile(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {"hbm_gbs": 6487.1, "bf16_tflops": 1736.2}
+    pk = peaks()                  # the same peaks as bench.py: MEASURED_PEAKS.json when present, else the H100 data sheet
     dev = "cuda"; tot = {"f": 0, "d": 0, "w": 0, "roof": 0}
-    print(f"B={B}  peak {pk['bf16_tflops']} TF (burst), {pk['hbm_gbs']} GB/s")
+    print(f"B={B}  {torch.cuda.get_device_name()}  peak {pk['tf_burst']} TF, {pk['hbm']} GB/s ({pk['src_tf']}; {pk['src_hbm']})")
     print(f"{'layer':22s} {'op':5s} {'ms':>8s} {'TF/s':>7s} {'GB/s':>7s} {'roof_ms':>8s} {'x_roof':>6s}")
     for name, cin, cout, k, s, p, hw, cnt in LAYERS:
         if only and only not in name: continue
@@ -47,7 +48,7 @@ def main():
         dy = torch.randn_like(y)
         flops = 2.0 * B * desc.p * desc.q * cout * cin * k * k
         bytes_io = 2.0 * (x.numel() + y.numel())
-        roof = max(flops / (pk["bf16_tflops"] * 1e12), bytes_io / (pk["hbm_gbs"] * 1e9)) * 1e3
+        roof = max(flops / (pk["tf_burst"] * 1e12), bytes_io / (pk["hbm"] * 1e9)) * 1e3
         for op, fn in (("fprop", lambda: ops.conv_fprop(desc, xn, wf)), ("dgrad", lambda: ops.conv_dgrad(desc, dy, wd)),
                        ("wgrad", lambda: ops.conv_wgrad(desc, xn, dy, m, cin))):
             t = timeit(fn)

@@ -1,4 +1,4 @@
-"""turboprune_b200 — B200-native (sm_100a) implementation of TurboPrune's masked-DDP hot path.
+"""turboprune_b200 — H100-native (sm_90a) implementation of TurboPrune's masked-DDP hot path.
 
 Host side mirrors the reference's surface (``utils.mask_layers``, ``utils.pruning_utils``,
 ``utils.custom_models``, ``harness_definitions``); the arithmetic runs in hand-written CUDA

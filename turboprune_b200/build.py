@@ -1,4 +1,4 @@
-"""Build the sm_100a CUDA library in-tree with nvcc (no JIT cache: the .so must travel with the repo)."""
+"""Build the sm_90a CUDA library in-tree with nvcc (no JIT cache: the .so must travel with the repo)."""
 import hashlib
 import os
 import shutil
@@ -11,7 +11,7 @@ LIBDIR = os.path.join(HERE, "lib")
 LIBNAME = "libturboprune_b200.so"
 SOURCES = ["tp_core.cu", "tp_prune.cu", "tp_optim.cu", "tp_igemm.cu", "tp_reduce.cu", "tp_bn.cu", "tp_pool.cu", "tp_data.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-cudart", "static",
 ]
 
@@ -25,7 +25,7 @@ def _nvcc() -> str:
     for cand in (os.environ.get("NVCC"), shutil.which("nvcc"), "/usr/local/cuda/bin/nvcc"):
         if cand and os.path.isfile(cand):
             return cand
-    raise RuntimeError("nvcc not found (needed to build turboprune_b200 for sm_100a)")
+    raise RuntimeError("nvcc not found (needed to build turboprune_b200 for sm_90a)")
 
 
 def _digest() -> str:
@@ -62,7 +62,7 @@ def build_variant(name: str, defines=()) -> str:
 
 
 def build(force: bool = False, verbose: bool = True) -> str:
-    """Compile every .cu for sm_100a and link lib/libturboprune_b200.so. Returns its path."""
+    """Compile every .cu for sm_90a and link lib/libturboprune_b200.so. Returns its path."""
     os.makedirs(LIBDIR, exist_ok=True)
     stamp = os.path.join(LIBDIR, "build.sha256")
     dig = _digest()

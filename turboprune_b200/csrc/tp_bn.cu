@@ -1,9 +1,8 @@
-// Fused BatchNorm (+ residual add) (+ ReLU) for NHWC bf16 activations, training and eval, sm_100a.
+// Fused BatchNorm (+ residual add) (+ ReLU) for NHWC bf16 activations, training and eval, sm_90a.
 //
 // SURVEY.md §8(f) row 1: the unmasked torchvision BatchNorm2d / ReLU / `out += identity` ops that sit
 // between every pair of masked convolutions (created at utils/custom_models.py:184 of the reference,
-// executed inside base_harness.py:124,127).  In the first profile they were 67 % of the step
-// (ATen batch_norm_* channels_last kernels run at ~0.5 TB/s); these kernels stream at HBM rate:
+// executed inside base_harness.py:124,127), in place of ATen's channels_last batch_norm_* kernels:
 //
 //   forward  : k_bn_stats (1 read)  -> k_bn_finalize_stats (tiny, fixed order => deterministic)
 //              -> k_bn_apply: z = relu(y*scale + shift (+ residual))            (1-2 reads, 1 write)
@@ -301,8 +300,7 @@ __global__ void __launch_bounds__(kBnThreads) k_bn_bwd_reduce(const __nv_bfloat1
     }
     const long long stride = (long long)gridDim.x * TY;
     long long p = (long long)blockIdx.x * TY + ty;
-    // 2 pixel rows in flight per thread (4-6 independent 16-byte loads); 4 rows measured SLOWER (6.9 -> 7.5 ms per step
-    // over the 53 layers): the extra registers cost more occupancy than the deeper queue buys
+    // 2 pixel rows in flight per thread (4-6 independent 16-byte loads); more rows cost registers, and with them occupancy
     constexpr int UR = 2;
     for (; p + (UR - 1) * stride < M; p += UR * stride) {
       uint4 vd[UR], vz[UR], vy[UR];

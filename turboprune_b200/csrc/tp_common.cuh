@@ -1,4 +1,4 @@
-// Shared helpers for the turboprune_b200 CUDA library (sm_100a only).
+// Shared helpers for the turboprune_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -33,9 +33,9 @@ inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 // previous grid is still finishing (as soon as every CTA of the previous grid has STARTED and executed
 // `griddepcontrol.launch_dependents`), and block in `griddepcontrol.wait` until that grid has completed and its memory
 // is visible.  Rules kept here: (1) a kernel launched through launch() executes pdl_wait() before its first global
-// access (pdl_enter() at the top, or after a prologue that touches only parameters / shared memory / TMEM);
+// access (pdl_enter() at the top, or after a prologue that touches only parameters / shared memory);
 // (2) the trigger comes first, so grids queue up behind each other only as deep as the SMs have room for.
-// Off by default (measured: a gain at small batches, a loss at batch 512 — see pdl_enabled()); TP_PDL=1 turns it on.
+// Off by default; TP_PDL=1 turns it on.
 bool pdl_enabled();
 #ifdef __CUDACC__
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

@@ -14,7 +14,6 @@ void set_last_cuda_error(cudaError_t e, const char* where) {
 
 static int g_pdl = -1;
 bool pdl_enabled() {
-  // measured (profiles/r02_notes.md, experiment 9): per-GPU batch 64: 7.68 -> 7.58 ms per step; batch 512: 42.14 -> 42.74 ms.
   // Opt-in (TP_PDL=1 or tp_set_pdl(1)) until the trigger placement is tuned per kernel.
   if (g_pdl < 0) { const char* e = getenv("TP_PDL"); g_pdl = (e && e[0] == '1') ? 1 : 0; }
   return g_pdl == 1;
@@ -23,10 +22,10 @@ bool pdl_enabled() {
 int sm_count() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cached[dev] = n;
   }
   return cached[dev];
@@ -98,7 +97,7 @@ const char* tp_strerror(int code) {
     case TP_ERR_CUDA: return "CUDA error (see tp_last_cuda_error)";
     case TP_ERR_K_RANGE: return "kthvalue(): selected number k out of range";
     case TP_ERR_UNSUPPORTED: return "unsupported configuration";
-    case TP_ERR_DEVICE: return "device is not sm_100 (B200)";
+    case TP_ERR_DEVICE: return "device is not sm_90 (H100)";
     default: return "unknown error";
   }
 }

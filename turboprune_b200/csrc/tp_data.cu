@@ -1,4 +1,4 @@
-// Data path either side of the model (SURVEY.md §8(f) row 3), sm_100a, HBM-bound:
+// Data path either side of the model (SURVEY.md §8(f) row 3), sm_90a, HBM-bound:
 //
 //   k_cifar_augment : the airbench-style GPU augmentation of the reference's CifarLoader.__iter__
 //                     (utils/dataset.py:192-226): random translate = batch_crop of the reflect-padded images (:43-69),

@@ -1,15 +1,15 @@
-// Masked implicit-GEMM convolution / linear for sm_100a: TMA (tiled + im2col) -> 128B-swizzled
-// shared memory -> tcgen05.mma (bf16 x bf16 -> fp32 in TMEM) -> tcgen05.ld epilogue.
+// Masked implicit-GEMM convolution / linear for sm_90a: TMA (tiled + im2col) -> 128B-swizzled
+// shared memory -> wgmma (bf16 x bf16 -> fp32 in registers) -> epilogue.
 //
 // Replaces F.conv2d / F.linear / F.conv1d(k=1) on the masked weight and their autograd
 // backward (utils/mask_layers.py:26-34, :70, :110-118 of the reference).  The mask never
 // appears here as a separate pass: fprop/dgrad consume bf16 weights that were masked while
 // being staged (tp_stage_weights), wgrad applies the mask in its finalize step.
 //
-// Two persistent, warp-specialised kernels (1 CTA / SM, 192 threads):
-//   warp 0     : TMA producer (one elected lane)
-//   warp 1     : TMEM allocator + tcgen05.mma issuer (one elected lane)
-//   warps 2..5 : epilogue (TMEM -> registers -> global), one TMEM lane quarter each
+// Two persistent, warp-specialised kernels (1 CTA / SM, 288 threads):
+//   warps 0..7 : two consumer warpgroups; warpgroup g issues the wgmma of rows 64g .. 64g+63 of the 128-row tile,
+//                then all eight warps run the epilogue
+//   warp 8     : TMA producer (one elected lane); runs ahead into the next tile while the epilogue drains
 //
 //   k_igemm_fwd  : D[pixels, Cout] = A[pixels, K] * W[Cout, K]^T          (fprop, dgrad)
 //                  A tile 128 pixels x 64 channels by TMA im2col (any r,s,stride,pad) or by
@@ -26,16 +26,18 @@
 namespace tp {
 using namespace ptx;
 
-constexpr int kBlockM = 128;         // UMMA M
+constexpr int kBlockM = 128;         // two wgmma M = 64 halves
 constexpr int kBlockK = 64;          // 64 bf16 = 128 B = one swizzle row
-constexpr int kThreads = 192;          // wgrad kernel: TMA warp, MMA warp, 4 epilogue warps
-constexpr int kFwdThreads = 320;       // fwd kernel: TMA warp, MMA warp, 8 epilogue warps (two per TMEM lane quarter)
+constexpr int kConsumers = 256;      // two consumer warpgroups
+constexpr int kThreads = kConsumers + 32;   // + the TMA producer warp (both kernels)
+constexpr int kProducerWarp = kConsumers / 32;
 constexpr int kMaxTaps = 64;
 
-// smem pipeline depth of the fwd kernel: stage = A tile (16 KB) + this CTA's share of the weight tile
-__host__ __device__ constexpr int fwd_stages(int block_n, int cl) {
-  return cl == 2 ? (block_n == 256 ? 6 : 8) : (block_n == 256 ? 4 : (block_n == 128 ? 6 : 8));
-}
+// smem pipeline depth of the fwd kernel: stage = A tile (16 KB) + weight tile (8 or 16 KB)
+__host__ __device__ constexpr int fwd_stages(int block_n) { return block_n == 128 ? 4 : 6; }
+// fwd smem besides the stages: fp32 accumulator exchange tile (128 x BLOCK_N), 8 x 4 KB epilogue staging, alignment
+// slack and barriers
+__host__ __device__ constexpr int fwd_tail(int block_n) { return kBlockM * block_n * 4 + 8 * 32 * 128 + 1024 + 512; }
 
 struct TapEntry { uint16_t off_w, off_h; int32_t kofs; };
 
@@ -51,7 +53,7 @@ struct ClsEntry {
   int ntaps, tap0;          // taps[tap0 .. tap0 + ntaps)
   int base_w, base_h;       // im2col coordinate of iteration pixel (p,q): base + q*step
   int oah, oaw;             // output pixel = (p*osh + oah, q*osw + oaw)
-  int tile0, m_groups;      // first work item of the class; M tile groups (of CL tiles) it has
+  int tile0, m_groups;      // first work item of the class; M tiles it has
 };
 
 struct FwdParams {
@@ -67,7 +69,6 @@ struct FwdParams {
   int linear;               // output pixel index == iteration pixel index (single class, unit output stride)
   int ws_stages, ws_b_bytes;   // weight-stationary instantiation: activation stages, bytes of the resident weight blocks
   int ldc;                  // elements between consecutive output pixels
-  int cluster;              // thread-block cluster size along M (1 or 2): weight tile multicast
   int tma_store;            // 1: epilogue stages 32x64 sub-tiles in smem and stores them with TMA (tmC)
   __nv_bfloat16* out;
   const float* bias;
@@ -147,16 +148,9 @@ __device__ __forceinline__ void decompose_pixel(int m, int P, int Q, int& n, int
 }
 
 // ============================================================================================
-// CL = 1: one CTA per 128 x BLOCK_N tile (tcgen05 cta_group::1).
-// CL = 2: a CTA PAIR (cluster of 2, tcgen05 cta_group::2) works on two neighbouring M tiles of the SAME N tile as one
-// 256 x BLOCK_N UMMA: each CTA loads its own 128-pixel A tile and only HALF of the weight tile (BLOCK_N/2 rows), the
-// leader CTA's MMA thread issues the pair MMAs (they read both CTAs' shared memory), each CTA's TMEM receives its
-// own 128 rows.  L2 -> SM operand bytes per K block drop from 2 x 48 KB to 2 x 32 KB and the 32 KB stages leave room
-// for 6 of them in flight: the ncu captures showed the mainloop pinned at ~10 TB/s of L2 -> SM traffic with every
-// role waiting (profiles/r01_notes.md); TMA multicast does not reduce L2 reads at cluster size 2, operand halving does.
 struct AMaps { CUtensorMap m[kMaxCls]; };      // activation-side tensor map of every class
 
-// work item -> (class, M-tile group, N tile); identical in the three roles
+// work item -> (class, M tile, N tile); identical in both roles
 __device__ __forceinline__ void decode_tile(const FwdParams& p, int tile, int n_tiles, int& c, int& m_g, int& n_t) {
   c = 0;
 #pragma unroll
@@ -165,36 +159,47 @@ __device__ __forceinline__ void decode_tile(const FwdParams& p, int tile, int n_
   m_g = local / n_tiles; n_t = local - m_g * n_tiles;     // m-major: CTAs running together share A tiles, weights stay in L2
 }
 
+// One warpgroup's share of a K block of the fwd GEMM: D[64 x BLOCK_N] (+)= A[64 x 64] * B[BLOCK_N x 64]^T, both K-major.
+template <int BLOCK_N>
+__device__ __forceinline__ void fwd_mma_block(float (&acc)[BLOCK_N / 2], uint32_t a_addr, uint32_t b_addr, uint32_t accumulate) {
+  const uint64_t adesc = make_smem_desc(a_addr, 16, 1024);
+  const uint64_t bdesc = make_smem_desc(b_addr, 16, 1024);
+#pragma unroll
+  for (int k = 0; k < kBlockK / 16; ++k) {
+    // advance 16 elements (32 B) along K inside the 128-B swizzle row: +2 in 16-B units
+    if constexpr (BLOCK_N == 128) wgmma_m64n128<0, 0>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), accumulate | (uint32_t)k);
+    else wgmma_m64n64<0, 0>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), accumulate | (uint32_t)k);
+  }
+}
+
 // MULTI = false: one class of output pixels (fprop, stride-1 dgrad) — the class decode, the per-row destination
-// arithmetic and the "class without taps" handling are compiled out (they cost the short-K layers up to 1.7x when they
-// sat in the common kernel: 1600 more instructions around loops that run once per 2-4 us tile).
+// arithmetic and the "class without taps" handling are compiled out.
 //
-// WS = true ("weight stationary", single class, CL = 1): when all K blocks of an output-channel tile fit in shared memory
-// next to a few activation stages (K x BLOCK_N x 2 B <= 144 KB: every 1x1 layer of ResNet-50's layer1-3, the 64-channel
-// 3x3s), a CTA keeps ONE output-channel tile for its whole life, loads its weight blocks once and then streams only
-// activation tiles.  The dense walk re-loaded BLOCK_N x 64 weights with every K block of every tile: for the 1x1 layers
-// that was 2/3 of the L2 -> SM operand traffic (128 of 192 KB per 128 x 256 x 256 tile) and it — not HBM, not the tensor
-// pipe — paced them (profiles/r01_notes.md: layer3 1x1 at 3.35 us per tile against 1.1 us of MMA and 1.9 us of HBM time).
+// WS = true ("weight stationary", single class): when all K blocks of an output-channel tile fit in shared memory next
+// to a few activation stages (the 1x1 layers of ResNet-50's layer1-3, the 64-channel 3x3s), a CTA keeps ONE
+// output-channel tile for its whole life, loads its weight blocks once and then streams only activation tiles (the
+// dense walk re-loads BLOCK_N x 64 weights with every K block of every tile).
 //
 // BNB = true (single class, linear output): the BatchNorm backward reduction of the layer that FEEDS this convolution is
 // done here, in the dgrad epilogue, instead of by k_bn_bwd_reduce (one read of dz and one of y per such layer less, one
 // launch less): after the bf16 gradient sub-tile has been staged, each lane re-reads it row-coalesced together with the
 // matching y values, applies the ReLU gate, stores g and adds sum(g), sum(g * xhat) of its 8 channels x 8 rows; rows are
 // then combined by the same fixed-order xor tree as the forward statistics.  Output: g, and [32-row group][2][N] partials.
-template <int BLOCK_N, int CL, bool MULTI, bool WS, bool BNB>
-__global__ void __launch_bounds__(kFwdThreads, 1)
+//
+// The accumulators leave the registers through an fp32 exchange tile in shared memory (16-byte chunk j of row r is
+// stored at chunk j ^ (r & 7): conflict-free for both the fragment stores and the row reads), so that each epilogue lane
+// owns one output row, as the coalesced staged stores and the 32-row statistics groups need.
+template <int BLOCK_N, bool MULTI, bool WS, bool BNB>
+__global__ void __launch_bounds__(kThreads, 1)
 k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ FwdParams p) {
-  static_assert(!WS || (CL == 1 && !MULTI), "weight-stationary walk: single CTA, single class");
-  static_assert(!BNB || (CL == 1 && !MULTI && !WS), "BatchNorm-backward epilogue: single CTA, single class, default walk");
+  static_assert(BLOCK_N == 64 || BLOCK_N == 128, "wgmma N of the fwd kernel");
+  static_assert(!WS || !MULTI, "weight-stationary walk: single class");
+  static_assert(!BNB || (!MULTI && !WS), "BatchNorm-backward epilogue: single class, default walk");
   constexpr int kABytes = kBlockM * kBlockK * 2;           // 16 KB
-  constexpr int kBRows = BLOCK_N / CL;                     // weight rows THIS CTA loads
-  constexpr int kBBytes = kBRows * kBlockK * 2;
+  constexpr int kBBytes = BLOCK_N * kBlockK * 2;
   constexpr int kStageBytes = kABytes + kBBytes;
-  constexpr int kStages = fwd_stages(BLOCK_N, CL);
-  constexpr int kAccStages = BLOCK_N == 256 ? 2 : 4;      // TMEM accumulator ring (512 columns at most)
-  constexpr uint32_t kTmemCols = (kAccStages * BLOCK_N <= 32) ? 32 : (kAccStages * BLOCK_N <= 64) ? 64 :
-                                 (kAccStages * BLOCK_N <= 128) ? 128 : (kAccStages * BLOCK_N <= 256) ? 256 : 512;
+  constexpr int kStages = fwd_stages(BLOCK_N);
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   pdl_trigger();
@@ -203,58 +208,42 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
   const int n_stages = WS ? p.ws_stages : kStages;         // WS: a stage is the 16 KB activation tile alone
   const int a_stride = WS ? kABytes : kStageBytes;
   uint8_t* const a_base = WS ? smem + p.ws_b_bytes : smem; // WS: the resident weight blocks come first
-  uint8_t* stg_base = a_base + n_stages * a_stride;        // 4 warps x 2 buffers x 4 KB (1024-B aligned)
+  float* const acc_tile = (float*)(a_base + n_stages * a_stride);     // 128 x BLOCK_N fp32
+  uint8_t* stg_base = (uint8_t*)(acc_tile + kBlockM * BLOCK_N);       // 8 warps x 4 KB (1024-B aligned)
   uint64_t* full_bar = (uint64_t*)(stg_base + 8 * kStgBytes);
   uint64_t* empty_bar = full_bar + (WS ? kMaxStages : kStages);
-  uint64_t* tfull_bar = empty_bar + (WS ? kMaxStages : kStages);
-  uint64_t* tempty_bar = tfull_bar + kAccStages;
-  uint64_t* bres_bar = tempty_bar + kAccStages;            // WS: the resident weight blocks have landed
-  uint32_t* tmem_slot = (uint32_t*)(bres_bar + 1);
+  uint64_t* bres_bar = empty_bar + (WS ? kMaxStages : kStages);       // WS: the resident weight blocks have landed
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_tiles = (p.N + BLOCK_N - 1) / BLOCK_N;
-  // work items are CLUSTER tiles: (class) x (group of CL neighbouring M tiles) x (N tile); CTA rank r takes M tile
-  // g*CL + r (an M tile past the end simply has no valid rows: its loads are zero-filled and its stores are masked)
-  const int cta_rank = (CL > 1) ? (int)cluster_ctarank() : 0;
-  const int cl_id = (int)blockIdx.x / CL, n_cl = (int)gridDim.x / CL;
+  // work items: (class) x (M tile) x (N tile), classes back to back
   const int total_tiles = p.cls[p.ncls - 1].tile0 + p.cls[p.ncls - 1].m_groups * n_tiles;
-  constexpr uint16_t kMask = (uint16_t)((1u << CL) - 1u);
   // the w-th work item of this CTA.  WS: one fixed N tile, M tiles ws_m0, ws_m0 + ws_dm, ... (CTAs with neighbouring ids
   // take the same M tile for the n_tiles different N tiles at about the same time: the activation tile comes from HBM once)
   const int ws_nt = WS ? (int)blockIdx.x % n_tiles : 0;
   const int ws_m0 = WS ? (int)blockIdx.x / n_tiles : 0, ws_dm = WS ? (int)gridDim.x / n_tiles : 1;
   const int my_items = WS ? (p.cls[0].m_groups > ws_m0 ? (p.cls[0].m_groups - ws_m0 + ws_dm - 1) / ws_dm : 0)
-                          : (total_tiles > cl_id ? (total_tiles - cl_id + n_cl - 1) / n_cl : 0);
+                          : (total_tiles > (int)blockIdx.x ? (total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0);
   auto get_tile = [&](int w, int& ci, int& m_g, int& n_t) {
     ci = 0;
     if (WS) { m_g = ws_m0 + w * ws_dm; n_t = ws_nt; return; }
-    const int tile = cl_id + w * n_cl;
+    const int tile = (int)blockIdx.x + w * (int)gridDim.x;
     if (MULTI) decode_tile(p, tile, n_tiles, ci, m_g, n_t);
     else { m_g = tile / n_tiles; n_t = tile - m_g * n_tiles; }   // m-major: CTAs running together share A tiles, weights stay in L2
   };
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int j = 0; j < p.ncls; ++j) prefetch_tmap(&tmA.m[j]);
     prefetch_tmap(&tmB);
-    // full / tempty are only used in the leader CTA of a pair: full gets ONE arrive (the leader's expect_tx for both
-    // CTAs' bytes), tempty gets one arrive per epilogue warp of both CTAs; empty / tfull exist in both CTAs and get
-    // one (multicast) commit arrival from the leader's MMA thread
-    for (int i = 0; i < n_stages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    for (int i = 0; i < kAccStages; ++i) { mbar_init(&tfull_bar[i], 1); mbar_init(&tempty_bar[i], 8 * CL); }
+    // empty: one arrival per consumer warpgroup once its MMAs have read the stage
+    for (int i = 0; i < n_stages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kConsumers / 128); }
     mbar_init(bres_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    if (CL == 1) { tmem_alloc(tmem_slot, kTmemCols); tmem_relinquish(); }
-    else { tmem_alloc_pair(tmem_slot, kTmemCols); tmem_relinquish_pair(); }
-  }
-  tc_fence_before();
-  if (CL > 1) cluster_sync_all(); else __syncthreads();      // peers' barriers are initialised before anyone signals them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();          // barriers, TMEM and descriptor prefetch above overlap the previous grid's tail; global memory from here on
+  __syncthreads();
+  pdl_wait();          // barrier set-up and descriptor prefetch above overlap the previous grid's tail; global memory from here on
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ------------------------------ TMA producer ------------------------------
     if (lane == 0) {
       int stage = 0; uint32_t phase = 0;
@@ -271,39 +260,25 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
         int ci, m_g, n_t; get_tile(w, ci, m_g, n_t);
         const ClsEntry& ce = p.cls[MULTI ? ci : 0];
         const CUtensorMap* const mapA = &tmA.m[MULTI ? ci : 0];
-        const int m_t = m_g * CL + cta_rank;
-        const int m0 = m_t * kBlockM;
+        const int m0 = m_g * kBlockM;
         int cn = 0, cp = 0, cq = 0;
         if (p.a_mode == 1) decompose_pixel(m0, ce.P_it, ce.Q_it, cn, cp, cq);
         const int cw = ce.base_w + cq * p.step_w, ch = ce.base_h + cp * p.step_h;
         auto load_block = [&](const TapEntry& te, int cc) {
-          mbar_wait(&empty_bar[stage], phase ^ 1, 1);
+          mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sA = a_base + stage * a_stride;
           uint8_t* sB = sA + kABytes;
-          if (CL == 1) {
-            mbar_arrive_expect_tx(&full_bar[stage], WS ? kABytes : kStageBytes);
-            if (p.a_mode == 1)
-              tma_load_im2col_4d(sA, mapA, &full_bar[stage], cc * kBlockK, cw, ch, cn, te.off_w, te.off_h);
-            else
-              tma_load_2d(sA, mapA, &full_bar[stage], te.kofs + cc * kBlockK, m0);
-            if (!WS) tma_load_2d(sB, &tmB, &full_bar[stage], te.kofs + cc * kBlockK, n_t * BLOCK_N);
-          } else {
-            // pair: my A tile and my half of the weight tile land in MY shared memory, the bytes are credited to the
-            // LEADER's full barrier (which expects both CTAs' stage bytes)
-            if (cta_rank == 0) mbar_arrive_expect_tx(&full_bar[stage], kStageBytes * CL);
-            const uint32_t lead_full = mapa_u32(smem_u32(&full_bar[stage]), 0);
-            if (p.a_mode == 1)
-              tma_load_im2col_4d_pair(sA, mapA, lead_full, cc * kBlockK, cw, ch, cn, te.off_w, te.off_h);
-            else
-              tma_load_2d_pair(sA, mapA, lead_full, te.kofs + cc * kBlockK, m0);
-            tma_load_2d_pair(sB, &tmB, lead_full, te.kofs + cc * kBlockK, n_t * BLOCK_N + cta_rank * kBRows);
-          }
+          mbar_arrive_expect_tx(&full_bar[stage], WS ? kABytes : kStageBytes);
+          if (p.a_mode == 1)
+            tma_load_im2col_4d(sA, mapA, &full_bar[stage], cc * kBlockK, cw, ch, cn, te.off_w, te.off_h);
+          else
+            tma_load_2d(sA, mapA, &full_bar[stage], te.kofs + cc * kBlockK, m0);
+          if (!WS) tma_load_2d(sB, &tmB, &full_bar[stage], te.kofs + cc * kBlockK, n_t * BLOCK_N);
           if (++stage == n_stages) { stage = 0; phase ^= 1; }
         };
         const int tap_base = MULTI ? ce.tap0 : 0;     // single class: a static table offset (no dependent parameter load)
         if (!km) {
           // dense walk — nested tap / channel-chunk loops: no integer division on the single producer thread
-          // (the first ncu source view showed the producer, not TMA or the tensor pipe, as the limiter)
           for (int tap = 0; tap < ce.ntaps; ++tap) {
             const TapEntry te = p.taps[tap_base + tap];
             for (int cc = 0; cc < p.cchunks; ++cc) load_block(te, cc);
@@ -324,82 +299,29 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer ------------------------------
-    if (lane == 0 && cta_rank == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(kBlockM * CL, BLOCK_N, 0, 0);
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      const uint32_t* const km = live_kmask(p.kmask, p.kmask_words, p.N);
-      if (WS && my_items > 0) { mbar_wait(bres_bar, 0, 5); tc_fence_after(); }
-      for (int w = 0; w < my_items; ++w) {
-        const int tile = cl_id + w * n_cl;      // (not used by the weight-stationary walk)
-        if (MULTI) {      // a class no tap reaches has no accumulator: its tiles belong to the epilogue warps alone
-          int ci0, mg0, nt0; decode_tile(p, tile, n_tiles, ci0, mg0, nt0);
-          if (p.cls[ci0].ntaps == 0) continue;
-        }
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1, 2);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BLOCK_N);
-        auto mma_block = [&](uint32_t accumulate, int kb) {
-          mbar_wait(&full_bar[stage], phase, 3);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(a_base + stage * a_stride);
-          const uint32_t b_addr = WS ? smem_u32(smem + kb * kBBytes) : a_addr + kABytes;   // WS: K block kb of the resident tile
-          const uint64_t adesc = make_smem_desc(a_addr, 16, 1024, kLayoutSW128);
-          const uint64_t bdesc = make_smem_desc(b_addr, 16, 1024, kLayoutSW128);
-#pragma unroll
-          for (int k = 0; k < kBlockK / 16; ++k) {
-            // advance 16 elements (32 B) along K inside the 128-B swizzle row: +2 in 16-B units
-            if (CL == 1) umma_bf16(d_tmem, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, accumulate | (uint32_t)k);
-            else umma_bf16_pair(d_tmem, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, accumulate | (uint32_t)k);
-          }
-          // frees this smem stage (in both CTAs of a pair) when the MMAs have read it
-          if (CL == 1) umma_commit(&empty_bar[stage]); else umma_commit_pair(&empty_bar[stage], kMask);
-          if (++stage == n_stages) { stage = 0; phase ^= 1; }
-        };
-        if (!MULTI && !km) {
-          // dense single-class walk: no tile arithmetic at all on this thread (it paces the tensor pipe)
-          const int kiters = p.cls[0].ntaps * p.cchunks;
-          for (int it = 0; it < kiters; ++it) mma_block((uint32_t)it, it);
-        } else {
-          int ci = 0, m_g = 0, n_t = 0;
-          if (MULTI) decode_tile(p, tile, n_tiles, ci, m_g, n_t); else n_t = WS ? ws_nt : tile % n_tiles;
-          const ClsEntry& ce = p.cls[MULTI ? ci : 0];       // a class without taps issues nothing: its epilogue writes the addend (or zero) alone
-          if (!km) {
-            const int kiters = ce.ntaps * p.cchunks;
-            for (int it = 0; it < kiters; ++it) mma_block((uint32_t)it, it);
-          } else {
-            KSkip ks; uint32_t any = 0;
-            ks.begin(km, p.kmask_words, n_t * BLOCK_N, BLOCK_N, p.N);
-            for (int tap = 0; tap < ce.ntaps; ++tap) {
-              const int kb0 = p.taps[(MULTI ? ce.tap0 : 0) + tap].kofs >> 6;
-              for (int cc = 0; cc < p.cchunks; ++cc) {
-                const bool last = tap == ce.ntaps - 1 && cc == p.cchunks - 1;
-                if (!ks.on(kb0 + cc) && !(last && !any)) continue;               // same decision as the producer
-                mma_block(any, tap * p.cchunks + cc);
-                any = 1;
-              }
-            }
-          }
-        }
-        // accumulator complete -> epilogue (of both CTAs of a pair)
-        if (CL == 1) umma_commit(&tfull_bar[acc]); else umma_commit_pair(&tfull_bar[acc], kMask);
-        if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
-      }
-    }
   } else {
-    // ------------------------------ epilogue ------------------------------
-    // 8 epilogue warps: the HBM-bound layers were limited by how fast 4 warps could drain TMEM (ncu: 3.5 TB/s of
-    // DRAM traffic at 30 % tensor activity).  Two warps share each TMEM lane quarter and split the columns.
-    const int quarter = warp & 3;             // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;         // which half of the 64-column chunks this warp drains
-    int acc = 0; uint32_t acc_phase = 0;
+    // ------------------------------ consumers: MMA, then epilogue ------------------------------
+    const int wg = warp >> 2;                 // MMA: rows 64*wg .. 64*wg+63 of the tile
+    const int quarter = warp & 3;             // epilogue: rows 32*quarter .. +31 of the tile, one per lane
+    const int half = warp >> 2;               // epilogue: which half of the 64-column chunks this warp drains
+    const int erow = quarter * 32 + lane;
+    int stage = 0; uint32_t phase = 0;
+    const uint32_t* const km = live_kmask(p.kmask, p.kmask_words, p.N);
+    if (WS && my_items > 0) mbar_wait(bres_bar, 0);
+    // 32 fp32 accumulators of this lane's row, columns c .. c+31, from the exchange tile
+    auto acc_row_ld = [&](int c, uint32_t* v) {
+      const uint32_t rb = smem_u32(acc_tile) + (uint32_t)(erow * BLOCK_N * 4);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const uint4 t = lds128(rb + ((uint32_t)(((c >> 2) + i) ^ (erow & 7)) << 4));
+        v[4 * i] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
+      }
+    };
     for (int w = 0; w < my_items; ++w) {
       int ci, m_g, n_t; get_tile(w, ci, m_g, n_t);
       const ClsEntry& ce = p.cls[MULTI ? ci : 0];
       const bool has_acc = MULTI ? ce.ntaps > 0 : true;   // a class no tap reaches: the accumulator was never written, its value is zero
-      const int m_t = m_g * CL + cta_rank;
+      const int m_t = m_g;
       const int row = m_t * kBlockM + quarter * 32 + lane;
       const bool row_ok = row < ce.M;
       long long opix = 0;
@@ -457,23 +379,65 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
         }
         continue;
       }
-      mbar_wait(&tfull_bar[acc], acc_phase, 4);
-      tc_fence_after();
-      const uint32_t t_base = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * BLOCK_N);
+      {
+        // ---- mainloop: this warpgroup's 64 x BLOCK_N accumulators over the tile's K blocks ----
+        float acc[BLOCK_N / 2];
+#pragma unroll
+        for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
+        int prev = -1;                        // stage of the previous K block: freed once its MMAs have completed
+        auto mma_block = [&](uint32_t accumulate, int kb) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint32_t s_addr = smem_u32(a_base + stage * a_stride);
+          const uint32_t b_addr = WS ? smem_u32(smem + kb * kBBytes) : s_addr + kABytes;   // WS: K block kb of the resident tile
+          wgmma_fence();
+          fwd_mma_block<BLOCK_N>(acc, s_addr + (uint32_t)(wg * (kABytes / 2)), b_addr, accumulate);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+          prev = stage;
+          if (++stage == n_stages) { stage = 0; phase ^= 1; }
+        };
+        // one walk with a single MMA call site (two would make ptxas serialise the wgmma pipeline)
+        KSkip ks; uint32_t any = 0;
+        if (km) ks.begin(km, p.kmask_words, n_t * BLOCK_N, BLOCK_N, p.N);
+        for (int tap = 0; tap < ce.ntaps; ++tap) {
+          const int kb0 = p.taps[(MULTI ? ce.tap0 : 0) + tap].kofs >> 6;
+          for (int cc = 0; cc < p.cchunks; ++cc) {
+            const bool last = tap == ce.ntaps - 1 && cc == p.cchunks - 1;
+            if (km && !ks.on(kb0 + cc) && !(last && !any)) continue;           // same decision as the producer
+            mma_block(any, tap * p.cchunks + cc);
+            any = 1;
+          }
+        }
+        wgmma_wait<0>();
+        acc_fence(acc);
+        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+        // ---- registers -> exchange tile (once the previous tile's epilogue has finished reading it) ----
+        bar_sync(1, kConsumers);
+        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = r0 + 8 * h, col = 8 * j + 2 * (lane & 3);
+            *reinterpret_cast<float2*>(acc_tile + r * BLOCK_N + (((col >> 2) ^ (r & 7)) << 2) + (col & 3)) =
+                make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+          }
+        bar_sync(1, kConsumers);
+      }
       if (p.tma_store) {
-        // TMEM -> registers -> 128B-swizzled smem sub-tile (32 rows x 64 cols) -> coalesced global
+        // accumulators -> registers -> 128B-swizzled smem sub-tile (32 rows x 64 cols) -> coalesced global
         // stores, so every output line leaves the SM as full 128-byte rows instead of 32 scattered 16-byte pieces.
         // Everything that does not depend on the column chunk is hoisted (row pointers, validity, swizzled
         // staging offsets) and the staging buffer is addressed through the shared window (st/ld.shared, not
-        // generic): the ncu source view of the first version had this loop at 2.3 us per 128x256 tile — longer
-        // than the tile's MMAs (1.1 us) — with its stalls on generic LD/ST and re-loaded kernel parameters.
-        const uint32_t buf = smem_u32(stg_base + (warp - 2) * kStgBytes);
+        // generic loads and stores, which are slower on shared memory).
+        const uint32_t buf = smem_u32(stg_base + warp * kStgBytes);
         __nv_bfloat16* const gout = p.out;
         const __nv_bfloat16* const gadd = p.addend;
         {
         const float* bias = p.bias;
         float* stats = p.stats ? p.stats + (long long)(m_t * 4 + quarter) * 2 * N + c16 * 8 : nullptr;
-        const uint32_t wr_base = buf + lane * 128;                              // my row (TMEM lane) in the staging tile
+        const uint32_t wr_base = buf + lane * 128;                              // my row in the staging tile
         const uint32_t wr_sw = (uint32_t)(lane & 7);
         const uint32_t rd_even = buf + r_in * 128 + ((uint32_t)(c16 ^ r_in) << 4);          // rows r_in + 8j
         const uint32_t rd_odd = buf + (r_in + 4) * 128 + ((uint32_t)(c16 ^ (r_in + 4)) << 4);  // rows r_in + 4 + 8j
@@ -485,8 +449,8 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
           const bool col_ok = n0 + c16 * 8 + 8 <= N;
           // both 32-column halves of the chunk are requested before the one wait
           uint32_t v[64];
-          tmem_ld_32x32(t_base + (uint32_t)c, v);
-          tmem_ld_32x32(t_base + (uint32_t)(c + 32), v + 32);
+          acc_row_ld(c, v);
+          acc_row_ld(c + 32, v + 32);
           if (gadd) {
             // addend sub-tile of THIS chunk was prefetched into registers one chunk earlier (coalesced: 8 lanes
             // cover one 128-byte row, 4 rows per instruction); stage it, then prefetch the next chunk's
@@ -509,7 +473,6 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
             }
             __syncwarp();
           }
-          tmem_ld_wait();
 #pragma unroll
           for (int j = 0; j < 64; j += 8) {
             float f[8];
@@ -539,7 +502,7 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
           __syncwarp();
           // smem -> global, coalesced: 8 lanes write one full 128-byte output row, 4 rows per instruction.
           // Plain stores are fire-and-forget, so the staging buffer is free again after this read-back
-          // (a TMA store here made every chunk wait ~2 us for the previous store to drain: 9 us per tile).
+          // (a TMA store here would make every chunk wait for the previous store to drain).
           uint4 o[8];
 #pragma unroll
           for (int i = 0; i < 8; ++i) o[i] = lds128(((i & 1) ? rd_odd : rd_even) + (uint32_t)((i >> 1) * 1024));
@@ -647,8 +610,7 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
 #pragma unroll 1
       for (int c = half * 32; c < BLOCK_N; c += 64) {
         uint32_t v[32];
-        tmem_ld_32x32(t_base + (uint32_t)c, v);
-        tmem_ld_wait();
+        acc_row_ld(c, v);
         const int n0 = n_t * BLOCK_N + c;
         if (row_ok && n0 < p.N) {
           float f[32];
@@ -680,24 +642,31 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
         }
       }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (CL == 1) mbar_arrive(&tempty_bar[acc]);
-        else mbar_arrive_cluster(mapa_u32(smem_u32(&tempty_bar[acc]), 0));     // the leader's MMA thread owns the accumulators
-      }
-      if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
     }
-  }
-  tc_fence_before();
-  if (CL > 1) cluster_sync_all(); else __syncthreads();      // nobody exits while the pair may still touch its smem / TMEM
-  if (warp == 1) {
-    tc_fence_after();
-    if (CL == 1) tmem_dealloc(tmem_base, kTmemCols); else tmem_dealloc_pair(tmem_base, kTmemCols);
   }
 }
 
 // ============================================================================================
+// One warpgroup's share of a K block of the wgrad GEMM: D[64 x NB*64] (+)= dY^T[64 couts x 64 pixels] *
+// Xcol[64 pixels x NB*64], both operands MN-major (64 MN elements per 128-B row, 8 pixel rows per 1024-B atom,
+// 64-column chunks 8 KB apart).
+template <int NB>
+__device__ __forceinline__ void wgrad_mma_block(float (&acc)[NB * 32], uint32_t a_addr, uint32_t b_addr, bool first) {
+  constexpr uint32_t kChunk = 64 * kBlockK * 2;
+#pragma unroll
+  for (int k = 0; k < kBlockK / 16; ++k) {
+    // 16 K rows = 2 swizzle atoms = 2048 B
+    const uint32_t acc_on = (!first || k > 0) ? 1u : 0u;
+    const uint64_t adesc = make_smem_desc(a_addr + (uint32_t)(2048 * k), kChunk, 1024);
+    const uint32_t bk = b_addr + (uint32_t)(2048 * k);
+    if constexpr (NB >= 2) wgmma_m64n128<1, 1>(acc, adesc, make_smem_desc(bk, kChunk, 1024), acc_on);
+    else wgmma_m64n64<1, 1>(acc, adesc, make_smem_desc(bk, kChunk, 1024), acc_on);
+    if constexpr (NB == 4) wgmma_m64n128<1, 1>(acc + 64, adesc, make_smem_desc(bk + 2 * kChunk, kChunk, 1024), acc_on);
+    if constexpr (NB == 3) wgmma_m64n64<1, 1>(acc + 64, adesc, make_smem_desc(bk + 2 * kChunk, kChunk, 1024), acc_on);
+  }
+}
+
+template <int NB>
 __global__ void __launch_bounds__(kThreads, 1)
 k_igemm_wgrad(const __grid_constant__ CUtensorMap tmA /* dY [Kpix, Cout] */,
               const __grid_constant__ CUtensorMap tmB /* X im2col or Xcol tiled */,
@@ -707,49 +676,40 @@ k_igemm_wgrad(const __grid_constant__ CUtensorMap tmA /* dY [Kpix, Cout] */,
   constexpr int kMaxNb = 4;
   constexpr int kStageBytes = kABytes + kMaxNb * kChunkBytes;   // 48 KB
   constexpr int kStages = 4;
-  constexpr uint32_t kTmemCols = 512;                     // 2 accumulator stages x 256 columns
   pdl_trigger();
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = (uint64_t*)(smem + kStages * kStageBytes);
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tfull_bar = empty_bar + kStages;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = (uint32_t*)(tempty_bar + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int items = p.m_tiles * p.n_tiles * p.splits;
-  const int ncols = p.nb * 64;
+  constexpr int ncols = NB * 64;
   const int row_groups = (p.Mc + 63) >> 6;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmA); prefetch_tmap(&tmB);
-    for (int i = 0; i < kStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull_bar[i], 1); mbar_init(&tempty_bar[i], 4); }
+    for (int i = 0; i < kStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kConsumers / 128); }
     fence_mbar_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_slot, kTmemCols); tmem_relinquish(); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();
   const uint32_t* const km = live_kmask(p.kmask, p.kmask_words, p.Mc);     // null: no empty block anywhere (or no mask given)
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     if (lane == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int item = blockIdx.x; item < items; item += gridDim.x) {
         // split-major order: the CTAs running at the same time work on the SAME pixel range for different
-        // (m, n) tiles, so each X / dY chunk comes from HBM once and from L2 for the siblings (ncu: 35.7 GB of
-        // DRAM reads per step with tile-major order vs ~23 GB algorithmic)
+        // (m, n) tiles, so each X / dY chunk comes from HBM once and from L2 for the siblings (tile-major order
+        // re-reads them from HBM)
         const int ntile = p.m_tiles * p.n_tiles;
         const int split = item / ntile, tile = item - split * ntile;
         const int n_t = tile / p.m_tiles, m_t = tile % p.m_tiles;
         const int kb0 = split * p.kb_per_split;
         const int kb1 = min(p.kblocks, kb0 + p.kb_per_split);
-        const int chunk0 = n_t * p.nb;
-        const int nvalid = min(p.nb, p.chunks - chunk0);
+        const int chunk0 = n_t * NB;
+        const int nvalid = min(NB, p.chunks - chunk0);
         if (km && wg_item_empty(km, p.kmask_words, row_groups, m_t, chunk0, nvalid)) continue;   // all three roles skip the same items
         // Everything that needs an integer division is hoisted out of the K loop (one producer thread
         // feeds the whole SM): per-chunk (tap, channel) coordinates once per item, and the pixel
@@ -764,7 +724,7 @@ k_igemm_wgrad(const __grid_constant__ CUtensorMap tmA /* dY [Kpix, Cout] */,
         const int sq = kBlockK % p.Q_it, t1 = kBlockK / p.Q_it, sp = t1 % p.P_it, sn = t1 / p.P_it;
         for (int kb = kb0; kb < kb1; ++kb) {
           const int pix0 = kb * kBlockK;
-          mbar_wait(&empty_bar[stage], phase ^ 1, 11);
+          mbar_wait(&empty_bar[stage], phase ^ 1);
           mbar_arrive_expect_tx(&full_bar[stage], kABytes + nvalid * kChunkBytes);
           uint8_t* sA = smem + stage * kStageBytes;
           uint8_t* sB = sA + kABytes;
@@ -788,82 +748,54 @@ k_igemm_wgrad(const __grid_constant__ CUtensorMap tmA /* dY [Kpix, Cout] */,
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(kBlockM, ncols, 1, 1);
-      int stage = 0; uint32_t phase = 0;
-      int acc = 0; uint32_t acc_phase = 0;
-      for (int item = blockIdx.x; item < items; item += gridDim.x) {
-        const int split = item / (p.m_tiles * p.n_tiles);
-        if (km) {
-          const int tile = item - split * (p.m_tiles * p.n_tiles), n_t = tile / p.m_tiles, m_t = tile - n_t * p.m_tiles;
-          if (wg_item_empty(km, p.kmask_words, row_groups, m_t, n_t * p.nb, min(p.nb, p.chunks - n_t * p.nb))) continue;
-        }
-        const int kb0 = split * p.kb_per_split;
-        const int kb1 = min(p.kblocks, kb0 + p.kb_per_split);
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1, 12);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * 256);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase, 13);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + stage * kStageBytes);
-          const uint32_t b_addr = a_addr + kABytes;
-          // MN-major SW128: 64 MN elements per 128-B row, 8 K rows per 1024-B atom (SBO),
-          // next 64-wide MN block at LBO = 64 rows * 128 B
-          const uint64_t adesc = make_smem_desc(a_addr, kChunkBytes, 1024, kLayoutSW128);
-          const uint64_t bdesc = make_smem_desc(b_addr, kChunkBytes, 1024, kLayoutSW128);
-#pragma unroll
-          for (int k = 0; k < kBlockK / 16; ++k) {
-            // 16 K rows = 2 swizzle atoms = 2048 B
-            umma_bf16(d_tmem, adesc + (uint64_t)(128 * k), bdesc + (uint64_t)(128 * k), idesc, (kb > kb0 || k > 0));
-          }
-          umma_commit(&empty_bar[stage]);
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tfull_bar[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
   } else {
-    const int quarter = warp & 3;
-    int acc = 0; uint32_t acc_phase = 0;
+    const int wg = warp >> 2;                 // rows (output channels) 64*wg .. 64*wg+63 of the tile
+    int stage = 0; uint32_t phase = 0;
     for (int item = blockIdx.x; item < items; item += gridDim.x) {
       const int ntile = p.m_tiles * p.n_tiles;
       const int split = item / ntile, tile = item - split * ntile;
       if (km) {
         const int n_t = tile / p.m_tiles, m_t = tile - n_t * p.m_tiles;
-        if (wg_item_empty(km, p.kmask_words, row_groups, m_t, n_t * p.nb, min(p.nb, p.chunks - n_t * p.nb))) continue;
+        if (wg_item_empty(km, p.kmask_words, row_groups, m_t, n_t * NB, min(NB, p.chunks - n_t * NB))) continue;
       }
-      float* prow = p.partial + (((long long)tile * p.splits + split) * kBlockM + quarter * 32 + lane) * ncols;
-      mbar_wait(&tfull_bar[acc], acc_phase, 14);
-      tc_fence_after();
-      const uint32_t t_base = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * 256);
-#pragma unroll 1
-      for (int c = 0; c < ncols; c += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(t_base + (uint32_t)c, v);
-        tmem_ld_wait();
+      const int kb0 = split * p.kb_per_split;
+      const int kb1 = min(p.kblocks, kb0 + p.kb_per_split);
+      float acc[NB * 32];
 #pragma unroll
-        for (int j = 0; j < 32; j += 4)
-          *(uint4*)(prow + c + j) = make_uint4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+      for (int i = 0; i < NB * 32; ++i) acc[i] = 0.f;
+      int prev = -1;                          // stage of the previous K block: freed once its MMAs have completed
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t a_addr = smem_u32(smem + stage * kStageBytes);
+        wgmma_fence();
+        wgrad_mma_block<NB>(acc, a_addr + (uint32_t)(wg * kChunkBytes), a_addr + kABytes, kb == kb0);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+      wgmma_wait<0>();
+      acc_fence(acc);
+      if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
+      // fragments -> fp32 partial tile [128][ncols]: 4 lanes write 32 contiguous bytes of a row
+      float* ptile = p.partial + ((long long)tile * p.splits + split) * kBlockM * ncols;
+      const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+      for (int j = 0; j < ncols / 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          *reinterpret_cast<float2*>(ptile + (long long)(r0 + 8 * h) * ncols + 8 * j + 2 * (lane & 3)) =
+              make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, kTmemCols); }
 }
 
 // dW[co][ci][tap] (fp32 OIHW) = mask * sum_split partial   — fixed summation order (deterministic, no atomics).
 // Grid (Cout, K chunks): a CTA owns KT = 256 / sl consecutive K columns (kk = tap*cin_p + ci) of one output channel;
 // its 256 threads are KT k-lanes x `sl` split-lanes.  Split lane j folds splits j, j+sl, ... with eight independent
 // loads in flight, the lanes are then combined in lane order.  (The first version looped over the K chunks inside one
-// CTA per channel: 18 dependent rounds of L2/DRAM latency for a 3x3x64 layer — 50-80 us for 150 KB of output.)
+// CTA per channel: 18 dependent rounds of L2/DRAM latency for a 3x3x64 layer.)
 __global__ void __launch_bounds__(256) k_wgrad_finalize(const float* __restrict__ partial, const float* __restrict__ mask,
                                                         float* __restrict__ dw, int cout, int cin_real, int cin_p, int rs,
                                                         int nb, int m_tiles, int n_tiles, int splits, int sl,
@@ -913,8 +845,8 @@ __global__ void __launch_bounds__(256) k_wgrad_finalize(const float* __restrict_
 // db[c] = sum over pixels of dy[pix][c]  (bias gradient), dy bf16 [npix, ldc], c % 8 == 0.
 // Two stages, both in fixed order (deterministic): every CTA of a (pixel split x channel tile) grid sums its pixels — a thread
 // owns one 16-byte vector of 8 channels and walks the pixel axis, 4 rows in flight — into part[split][c]; a small kernel
-// folds the splits.  (The first version ran ONE CTA per 32 channels over all pixels with 2-byte loads: 200 us per layer —
-// 41 % of the DeiT-S step, profiles/r02_launches_deit_B64.md.)
+// folds the splits.  (The first version ran ONE CTA per 32 channels over all pixels with 2-byte loads: most of the DeiT-S
+// step.)
 __global__ void __launch_bounds__(256) k_colsum_part(const __nv_bfloat16* __restrict__ dy, long long npix, int c, int ldc,
                                                      float* __restrict__ part) {
   pdl_enter();
@@ -1046,7 +978,7 @@ static int make_im2col_map(CUtensorMap* m, const void* ptr, int n, int h, int w,
   return TP_OK;
 }
 
-// Split-K factor of the wgrad GEMM.  Every (tile, split) item costs its share of the K loop plus a fixed 128 x 256
+// Split-K factor of the wgrad GEMM.  Every (tile, split) item costs its share of the K loop plus a fixed 128 x nb*64
 // fp32 partial tile (written once, read once by the finalize pass), so the cheapest choice is the SMALLEST split
 // count that reaches the minimal makespan over the persistent CTAs — not "as many as fit in two waves": at a per-GPU
 // batch of 64 the partial tiles were most of the wgrad traffic (54 layers x ~300 items x 128 KB, twice).
@@ -1055,9 +987,15 @@ static int pick_wgrad_splits(int tiles, int kblocks, int nb) {
   int smax = (2 * sms) / tiles;
   if (smax > kblocks) smax = kblocks;
   if (smax < 1) smax = 1;
-  const double c_kb = 0.30;                         // us per 64-pixel K block (48 KB of operands, one 128x256x64 MMA group)
-  const double c_part = 0.33 * nb;                  // us to drain one partial tile from TMEM to global
-  const double c_fin = 0.013 * nb;                  // us of finalize traffic per partial tile (read once at ~5 TB/s)
+  // Relative costs (only their ratios decide): a 64-pixel K block (48 KB of operands, one 128 x nb*64 x 64 MMA group),
+  // storing one partial tile from the accumulator registers to global, and the finalize traffic of one partial tile.
+  // These weights were calibrated on an earlier GPU generation (where the partial tile was drained through tensor memory)
+  // and are NOT re-fitted for H100.  Checked on an H100 SXM (700 W) by sweeping the split count of every ResNet-50 wgrad
+  // layer: the splits chosen here cost 7.6 % (batch 512) and 6.4 % (batch 64) more wgrad + finalize time than the best
+  // split of each layer; the model fills exactly one wave, while the measured optima scatter around it.
+  const double c_kb = 0.30;
+  const double c_part = 0.33 * nb;
+  const double c_fin = 0.013 * nb;
   int best = 1; double best_cost = 1e30;
   for (int s = 1; s <= smax; ++s) {
     const int kb = (kblocks + s - 1) / s;
@@ -1075,16 +1013,18 @@ static bool is_plain_gemm(const tp_conv_desc* d) {
 }
 
 static int pick_block_n(long long m_tiles, int n) {
-  // favour wide tiles (fewer re-reads of the activation tile), but keep the last wave full
+  // favour wide tiles (fewer re-reads of the activation tile), but keep the last wave full.  128 is the widest tile:
+  // a warpgroup holds its 64 x BLOCK_N fp32 accumulators in registers, and the 128 x BLOCK_N exchange tile plus four
+  // 32 KB stages fill the 227 KB of shared memory.
   const int sms = sm_count();
   if (const char* e = getenv("TP_IGEMM_BN")) {        // experiments only: force the tile width
     const int f = atoi(e);
-    if ((f == 64 || f == 128 || f == 256) && (f == 64 || n > f / 2)) return f;
+    if ((f == 64 || f == 128) && (f == 64 || n > f / 2)) return f;
   }
   int best = 64; double best_score = -1;
-  const int cands[3] = {256, 128, 64};
-  const double weight[3] = {1.0, 0.92, 0.75};
-  for (int i = 0; i < 3; ++i) {
+  const int cands[2] = {128, 64};
+  const double weight[2] = {1.0, 0.82};
+  for (int i = 0; i < 2; ++i) {
     int bn = cands[i];
     if (bn > 64 && n <= bn / 2) continue;
     long long tiles = m_tiles * ((n + bn - 1) / bn);
@@ -1095,49 +1035,40 @@ static int pick_block_n(long long m_tiles, int n) {
   return best;
 }
 
-constexpr int kSmemMax = 232448;                 // 227 KB: the per-CTA opt-in limit of sm_100
-constexpr int kWsMaxBBytes = 144 * 1024;         // resident weight blocks of the weight-stationary walk
+constexpr int kSmemMax = 232448;                 // 227 KB: the per-CTA opt-in limit of sm_90
+constexpr int kWsMinStages = 3;                  // activation stages the weight-stationary walk keeps in flight at least
 
-template <int BN, int CL, bool MULTI, bool WS, bool BNB = false>
+template <int BN, bool MULTI, bool WS, bool BNB = false>
 static int launch_fwd(const AMaps& a, const CUtensorMap& b, FwdParams& p, cudaStream_t st) {
-  constexpr int kStages = fwd_stages(BN, CL);
-  constexpr int kTail = 8 * 32 * 128 + 1024 + 512;    // epilogue staging, alignment slack, barriers
-  int smem = kStages * (kBlockM * kBlockK * 2 + (BN / CL) * kBlockK * 2) + kTail;
+  constexpr int kStages = fwd_stages(BN);
+  constexpr int kTail = fwd_tail(BN);
+  int smem = kStages * (kBlockM * kBlockK * 2 + BN * kBlockK * 2) + kTail;
+  static_assert(fwd_stages(BN) * (kBlockM * kBlockK * 2 + BN * kBlockK * 2) + fwd_tail(BN) <= kSmemMax, "fwd smem budget");
   const int n_tiles = (p.N + BN - 1) / BN;
   if (WS) {
     p.ws_b_bytes = p.cls[0].ntaps * p.cchunks * BN * kBlockK * 2;
     p.ws_stages = (kSmemMax - kTail - p.ws_b_bytes) / (kBlockM * kBlockK * 2);
     if (p.ws_stages > 16) p.ws_stages = 16;
-    if (p.ws_stages < 3) return TP_ERR_UNSUPPORTED;
+    if (p.ws_stages < kWsMinStages) return TP_ERR_UNSUPPORTED;
     smem = p.ws_b_bytes + p.ws_stages * kBlockM * kBlockK * 2 + kTail;
   }
   static bool attr_set = false;
   if (!attr_set) {
-    TP_CUDA_CHECK(cudaFuncSetAttribute(k_igemm_fwd<BN, CL, MULTI, WS, BNB>, cudaFuncAttributeMaxDynamicSharedMemorySize, WS ? kSmemMax : smem));
+    TP_CUDA_CHECK(cudaFuncSetAttribute(k_igemm_fwd<BN, MULTI, WS, BNB>, cudaFuncAttributeMaxDynamicSharedMemorySize, WS ? kSmemMax : smem));
     attr_set = true;
   }
-  // work items: per class, (groups of CL M tiles) x (N tiles), classes back to back
+  // work items: per class, (M tiles) x (N tiles), classes back to back
   long long ctiles = 0;
   for (int c = 0; c < p.ncls; ++c) {
-    const long long m_tiles = (p.cls[c].M + kBlockM - 1) / kBlockM;
-    p.cls[c].m_groups = (int)((m_tiles + CL - 1) / CL);
+    p.cls[c].m_groups = (int)((p.cls[c].M + kBlockM - 1) / kBlockM);
     if (ctiles > 0x7fffffffll) return TP_ERR_UNSUPPORTED;
     p.cls[c].tile0 = (int)ctiles;
     ctiles += (long long)p.cls[c].m_groups * n_tiles;
   }
   if (ctiles > 0x7fffffffll || ctiles <= 0) return TP_ERR_UNSUPPORTED;
-  const long long max_cl = sm_count() / CL;
-  int grid = (int)(ctiles < max_cl ? ctiles : max_cl) * CL;
+  int grid = (int)(ctiles < sm_count() ? ctiles : sm_count());
   if (WS) grid = (sm_count() / n_tiles) * n_tiles;           // every CTA owns one N tile: a whole number of CTAs per N tile
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kFwdThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = (CL == 1 && pdl_enabled()) ? 2 : 1;     // pairs stay fully serialised
-  TP_CUDA_CHECK(cudaLaunchKernelEx(&cfg, k_igemm_fwd<BN, CL, MULTI, WS, BNB>, a, b, p));
+  TP_CUDA_CHECK(launch(k_igemm_fwd<BN, MULTI, WS, BNB>, dim3(grid), dim3(kThreads), (size_t)smem, st, a, b, p));
   TP_LAUNCH_CHECK();
   return TP_OK;
 }
@@ -1154,58 +1085,42 @@ static int run_fwd(const AMaps& a, const CUtensorMap& b, FwdParams& p, int bn, c
   // the iteration order itself
   const bool multi = !p.linear;
   if (multi) {
-    if (p.cluster == 2) {
-      if (bn == 256) return launch_fwd<256, 2, true, false>(a, b, p, st);
-      if (bn == 128) return launch_fwd<128, 2, true, false>(a, b, p, st);
-      return launch_fwd<64, 2, true, false>(a, b, p, st);
-    }
-    if (bn == 256) return launch_fwd<256, 1, true, false>(a, b, p, st);
-    if (bn == 128) return launch_fwd<128, 1, true, false>(a, b, p, st);
-    return launch_fwd<64, 1, true, false>(a, b, p, st);
-  }
-  if (p.cluster == 2) {
-    if (bn == 256) return launch_fwd<256, 2, false, false>(a, b, p, st);
-    if (bn == 128) return launch_fwd<128, 2, false, false>(a, b, p, st);
-    return launch_fwd<64, 2, false, false>(a, b, p, st);
+    if (bn == 128) return launch_fwd<128, true, false>(a, b, p, st);
+    return launch_fwd<64, true, false>(a, b, p, st);
   }
   if (p.bn_y) {      // BatchNorm-backward epilogue (needs the linear staged path; the caller checked the shapes)
     if (!p.tma_store || !p.stats) return TP_ERR_UNSUPPORTED;
-    if (bn == 256) return launch_fwd<256, 1, false, false, true>(a, b, p, st);
-    if (bn == 128) return launch_fwd<128, 1, false, false, true>(a, b, p, st);
-    return launch_fwd<64, 1, false, false, true>(a, b, p, st);
+    if (bn == 128) return launch_fwd<128, false, false, true>(a, b, p, st);
+    return launch_fwd<64, false, false, true>(a, b, p, st);
   }
   // weight-stationary walk: the tile's weight blocks fit next to >= 3 activation stages, there is a whole number of CTAs
-  // per N tile and enough M tiles for every CTA to amortise the one-time weight load
+  // per N tile and enough M tiles for every CTA to amortise the one-time weight load.  Opt-in (TP_IGEMM_WS=1),
+  // parity-tested against the default walk.
   const int n_tiles = (p.N + bn - 1) / bn;
   const long long m_tiles = (p.cls[0].M + kBlockM - 1) / kBlockM;
   const long long b_bytes = (long long)p.cls[0].ntaps * p.cchunks * bn * kBlockK * 2;
-  // Measured on B200 (profiles/r02_notes.md, conv_bench at B = 512): bit-identical, but only 0-5 % faster on the layer3
-  // 1x1s and 5-8 % SLOWER on layer1's (fewer bytes in flight per SM with 16 KB stages) — like the cta_group::2 pair kernel
-  // of round 1 this says the weight bytes crossing L2 -> SM are not what paces these layers.  Opt-in (TP_IGEMM_WS=1),
-  // parity-tested.
+  const long long ws_max_b = (long long)kSmemMax - (bn == 128 ? fwd_tail(128) : fwd_tail(64)) - kWsMinStages * kBlockM * kBlockK * 2;
   const char* e = getenv("TP_IGEMM_WS");
-  const bool ws = e && atoi(e) != 0 && b_bytes <= kWsMaxBBytes && n_tiles <= sm_count() / 2 && m_tiles >= 4ll * (sm_count() / n_tiles);
+  const bool ws = e && atoi(e) != 0 && b_bytes <= ws_max_b && n_tiles <= sm_count() / 2 && m_tiles >= 4ll * (sm_count() / n_tiles);
   if (ws) {
-    if (bn == 256) return launch_fwd<256, 1, false, true>(a, b, p, st);
-    if (bn == 128) return launch_fwd<128, 1, false, true>(a, b, p, st);
-    return launch_fwd<64, 1, false, true>(a, b, p, st);
+    if (bn == 128) return launch_fwd<128, false, true>(a, b, p, st);
+    return launch_fwd<64, false, true>(a, b, p, st);
   }
-  if (bn == 256) return launch_fwd<256, 1, false, false>(a, b, p, st);
-  if (bn == 128) return launch_fwd<128, 1, false, false>(a, b, p, st);
-  return launch_fwd<64, 1, false, false>(a, b, p, st);
+  if (bn == 128) return launch_fwd<128, false, false>(a, b, p, st);
+  return launch_fwd<64, false, false>(a, b, p, st);
 }
 
-// Cluster size for a problem: pairs of M tiles share the weight tile (multicast) whenever there are enough tiles.
-static int pick_cluster(long long m_tiles) {
-  const char* e = getenv("TP_IGEMM_CLUSTER");        // read every call: the parity tests flip it
-  const int forced = e ? atoi(e) : 0;
-  if (forced == 1 || forced == 2) return forced;
-  // Measured on B200 (profiles/r01_notes.md, tools/conv_bench.py): the cta_group::2 pair kernel is bit-identical but
-  // not faster — 0.92-0.96x on the layer4 GEMMs, 1.05-1.4x SLOWER on the HBM-bound layers (both CTAs' epilogues and
-  // loads gate every accumulator hand-off through cluster-remote arrivals).  The mainloop is not L2-bandwidth bound,
-  // the per-tile epilogue is.  Pairs stay selectable with TP_IGEMM_CLUSTER=2 (parity-tested).
-  (void)m_tiles;
-  return 1;
+template <int NB>
+static int launch_wgrad(int grid, const CUtensorMap& ta, const CUtensorMap& tb, const WgParams& p, cudaStream_t st) {
+  constexpr int smem = 4 * (kBlockM * kBlockK * 2 + 4 * 64 * kBlockK * 2) + 1024 + 256;
+  static bool attr_set = false;
+  if (!attr_set) {
+    TP_CUDA_CHECK(cudaFuncSetAttribute(k_igemm_wgrad<NB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    attr_set = true;
+  }
+  TP_CUDA_CHECK(launch(k_igemm_wgrad<NB>, dim3(grid), dim3(kThreads), (size_t)smem, st, ta, tb, p));
+  TP_LAUNCH_CHECK();
+  return TP_OK;
 }
 
 }  // namespace tp
@@ -1281,8 +1196,7 @@ int tp_conv_fprop_stats(const tp_conv_desc* d, const void* x, const void* wf, co
   }
   for (int c = 1; c < kMaxCls; ++c) ta.m[c] = ta.m[0];
   const int bn = pick_block_n((p.M + kBlockM - 1) / kBlockM, p.N);
-  p.cluster = pick_cluster((p.M + kBlockM - 1) / kBlockM);
-  rc = make_tiled_map(&tb, wf, (uint64_t)d->r * d->s * d->cin, (uint64_t)d->cout, (uint64_t)d->r * d->s * d->cin, (uint32_t)(bn / p.cluster));
+  rc = make_tiled_map(&tb, wf, (uint64_t)d->r * d->s * d->cin, (uint64_t)d->cout, (uint64_t)d->r * d->s * d->cin, (uint32_t)bn);
   if (rc) return rc;
   return run_fwd(ta, tb, p, bn, st);
 }
@@ -1362,8 +1276,8 @@ static int conv_dgrad_impl(const tp_conv_desc* d, const void* dy, const void* wd
     for (int c = 1; c < kMaxCls; ++c) ta.m[c] = ta.m[0];
   } else {
     // strided conv: dX splits into stride_h x stride_w parity classes; each class is a stride-1 gather over dY with its
-    // own subset of taps, written to every stride-th pixel.  ONE launch covers all classes (round 1: a memset / memcpy
-    // of dX plus one launch per class with scattered 16-byte stores — 2.5-4x the roofline of these layers); a class
+    // own subset of taps, written to every stride-th pixel.  ONE launch covers all classes (no memset / memcpy of dX,
+    // no launch per class with scattered 16-byte stores); a class
     // no tap reaches is written by the epilogue alone (the fused addend, or zero).
     if (sh * sw > kMaxCls || R * S > kMaxTaps) return TP_ERR_UNSUPPORTED;
     p.a_mode = 1; p.osh = sh; p.osw = sw;
@@ -1401,8 +1315,7 @@ static int conv_dgrad_impl(const tp_conv_desc* d, const void* dy, const void* wd
   long long m_tiles = 0;
   for (int c = 0; c < p.ncls; ++c) m_tiles += (p.cls[c].M + kBlockM - 1) / kBlockM;
   const int bn = pick_block_n(m_tiles, p.N);
-  p.cluster = pick_cluster(m_tiles);
-  rc = make_tiled_map(&tb, wd, (uint64_t)ktot, (uint64_t)d->cin, (uint64_t)ktot, (uint32_t)(bn / p.cluster)); if (rc) return rc;
+  rc = make_tiled_map(&tb, wd, (uint64_t)ktot, (uint64_t)d->cin, (uint64_t)ktot, (uint32_t)bn); if (rc) return rc;
   return run_fwd(ta, tb, p, bn, st);
 }
 
@@ -1450,15 +1363,15 @@ int tp_conv_wgrad(const tp_conv_desc* d, const void* x, const void* dy, const vo
     rc = make_im2col_map(&tb, x, d->n, d->h, d->w, d->cin, p.base_w, p.base_h, p.step_w, p.step_h, d->p, d->q, 64);
     if (rc) return rc;
   }
-  constexpr int smem = 4 * (kBlockM * kBlockK * 2 + 4 * 64 * kBlockK * 2) + 1024 + 256;
-  static bool attr_set = false;
-  if (!attr_set) {
-    TP_CUDA_CHECK(cudaFuncSetAttribute(k_igemm_wgrad, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr_set = true;
-  }
   const int items = p.m_tiles * p.n_tiles * splits;
-  launch(k_igemm_wgrad, items < sms ? items : sms, kThreads, smem, st, ta, tb, p);
-  TP_LAUNCH_CHECK();
+  const int grid = items < sms ? items : sms;
+  switch (p.nb) {
+    case 1: rc = launch_wgrad<1>(grid, ta, tb, p, st); break;
+    case 2: rc = launch_wgrad<2>(grid, ta, tb, p, st); break;
+    case 3: rc = launch_wgrad<3>(grid, ta, tb, p, st); break;
+    default: rc = launch_wgrad<4>(grid, ta, tb, p, st); break;
+  }
+  if (rc) return rc;
   // split lanes only pay when there are many splits (skinny layers); wide-K layers keep all 256 threads on K
   const int sl = splits >= 64 ? 8 : (splits >= 32 ? 4 : (splits >= 16 ? 2 : 1));
   const int fin_kt = 256 / sl;

@@ -12,8 +12,8 @@ namespace tp {
 // output channel through shared memory so both the read and the wf write are coalesced.
 // One CTA stages a tile of kCoT output channels x a slice of input channels: the [co][ci][tap] slab goes through shared
 // memory so that the OIHW read, the wf write (channels contiguous per tap) and the wd write (kCoT output channels =
-// one 16-byte store per (ci, tap)) are all coalesced.  (Staging one output channel per CTA made every wd element a
-// separate 2-byte sector write: 0.32 ms for the 25.5 M weights of ResNet-50 instead of ~0.08 ms.)
+// one 16-byte store per (ci, tap)) are all coalesced.  (Staging one output channel per CTA makes every wd element a
+// separate 2-byte sector write.)
 constexpr int kCoT = 8;
 constexpr int kSlabFloats = 8192;            // 32 KB
 
@@ -126,7 +126,7 @@ __global__ void __launch_bounds__(256) k_stage_weights(const float* __restrict__
   stage_slab(w, mask, blockIdx.x * kCoT, cout, c0, c1, cin, rs, wf, cin_p, wf_ld, wd, cout_p, true, s_slab, kmf, kmf_words, kmd, kmd_words);
 }
 
-// All masked layers of a model in ONE launch (54 launches of ~10 us each were 5 % of the per-GPU-batch-64 step).
+// All masked layers of a model in ONE launch instead of one launch per layer (54 for ResNet-50).
 // The operand buffers are persistent and zero-initialised by the host, so channel padding is never rewritten.
 struct StageItem {
   const float* w; const float* mask; __nv_bfloat16* wf; __nv_bfloat16* wd;
@@ -293,7 +293,7 @@ __global__ void __launch_bounds__(256) k_im2col_stem(const T* __restrict__ src, 
 // shared memory as bf16 (coalesced reads, padding resolved there), then every 16-byte cell of the strip's rows is a gather
 // of 8 halfwords from shared memory with loop-invariant offsets (thread = one cell column, walking the strip's pixels).
 // The per-cell kernel above spends its time on 8 bounds-checked scalar global loads + 8 table lookups + 3 divisions per
-// cell: 1.45 ms per B = 512 step for 2.26 GB of traffic (1.6 TB/s); this one has none of them in the inner loop.
+// cell; this one has none of them in the inner loop.
 template <typename T>
 __global__ void __launch_bounds__(256) k_im2col_stem_rows(const T* __restrict__ src, long long sn, long long sc, long long sh, long long sw,
                                                           int n, int c, int h, int w, int R, int S, int cg, int stride_h, int stride_w,

@@ -1,7 +1,6 @@
-// Max pooling (forward with saved arg-max, backward) for NHWC bf16 activations, sm_100a.
+// Max pooling (forward with saved arg-max, backward) for NHWC bf16 activations, sm_90a.
 // The torchvision stem's MaxPool2d(3, 2, 1) sits between the first masked conv block and layer1
-// (SURVEY.md §8(f) row 1: unmasked neighbours of the masked convs); ATen's NHWC kernels took 4.9 ms
-// per B=512 step (max_pool_backward_nhwc alone 3.4 ms), these stream at HBM rate.
+// (SURVEY.md §8(f) row 1: unmasked neighbours of the masked convs); these kernels replace ATen's NHWC max pooling.
 //   forward : one thread per (output pixel, 8 channels): 16-byte loads over the window, -inf padding,
 //             NaN propagates (torch semantics), first maximum wins; writes y and a uint8 window index
 //   backward: gather form (no atomics, deterministic): one thread per (input pixel, 8 channels) sums dy
@@ -99,8 +98,8 @@ __global__ void __launch_bounds__(256) k_maxpool_bwd(const __nv_bfloat16* __rest
 }
 
 // ---- MaxPool2d(3, 2, 1) — the torchvision ResNet stem — with the geometry known at compile time: every tap is a predicated
-// 16-byte load issued before the first compare (the generic kernels walk runtime-bounded loops: 1.02 ms backward / 0.47 ms
-// forward per B = 512 step for 1.1 GB of traffic, i.e. 1.1 / 2.4 TB/s).  Same tap order, same arg-max rule, same rounding.
+// 16-byte load issued before the first compare (the generic kernels walk runtime-bounded loops).  Same tap order, same
+// arg-max rule, same rounding.
 __global__ void __launch_bounds__(256) k_maxpool_fwd_321(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y,
                                                          unsigned char* __restrict__ idx, int n, int h, int w, int c, int p, int q) {
   pdl_enter();

@@ -1,4 +1,4 @@
-// Pruning score -> exact global k-th smallest -> mask, for sm_100a.
+// Pruning score -> exact global k-th smallest -> mask, for sm_90a.
 //
 // Replaces utils/pruning_utils.py:73-87 / :186-203 / :263-283 of the reference
 // (per-layer score temporaries, torch.cat, single-CTA 16-pass torch.kthvalue, per-layer
@@ -16,8 +16,7 @@
 //   P5 finish   : every CTA selects the exact key among those in shared memory (no further barrier), patches its
 //                 share of the candidates' masks; CTA 0 publishes threshold and status.
 //
-// (Round 1 ran this as six kernels + a blocking status read-back: 158 us for ResNet-50's 25.5 M weights of which the
-// sweep was 60 us.)  If the bracket misses (adversarial ties, overflow of a list) the status says so and the host
+// If the bracket misses (adversarial ties, overflow of a list) the status says so and the host
 // runs an exact 3-pass 11/11/10-bit radix select over the full data + one apply pass — tp_topk_finish, which is
 // also where the status is read back, so the fast path itself never blocks the stream.
 // Both paths are bit-exact with torch.kthvalue + torch.where(score <= thr, 0, 1).
@@ -210,8 +209,8 @@ __global__ void __launch_bounds__(kSweepThreads) k_topk_fused(const TopkArgs a) 
   for (int i = t; i < kDigitBins; i += kSweepThreads) s_h[i] = 0;
   __syncthreads();
   // samples are taken in runs of kRun = 16 neighbouring elements: one 64-byte DRAM burst per operand serves 16 samples.
-  // (Runs of 4 — one 32-byte sector — made this phase 28 us for ResNet-50: 2 x 262144 scattered sectors is a random-access
-  // rate problem, not a bandwidth one; the host widens the rank band for the clustering.)
+  // (Runs of 4 — one 32-byte sector — turn sampling into a random-access rate problem rather than a bandwidth one; the
+  // host widens the rank band for the clustering.)
   const long long G = (a.S + kRun - 1) / kRun;
   const long long first = blockIdx.x * (long long)kSweepThreads, gstride = (long long)gridDim.x * kSweepThreads;
   const int rounds = first < G ? (int)((G - first + gstride - 1) / gstride) : 0;   // uniform over the CTA; host keeps rounds * 256 * kRun <= kLocalKeys
@@ -252,9 +251,8 @@ __global__ void __launch_bounds__(kSweepThreads) k_topk_fused(const TopkArgs a) 
       *reinterpret_cast<uint4*>(&s_keys[((r * kSweepThreads + t) * kRun) + 4 * q]) = make_uint4(key[4 * q], key[4 * q + 1], key[4 * q + 2], key[4 * q + 3]);
   }
   __syncthreads();
-  // (Tried: asking the L2 for this CTA's first 2-8 sweep tiles here with cp.async.bulk.prefetch.L2 while the sample is being
-  // resolved.  The sweep got 2-8 us shorter, but this phase 4-21 us longer — the histogram atomics and the grid barrier
-  // queue behind the prefetch traffic.  profiles/r02_notes.md.)
+  // (No L2 prefetch of this CTA's first sweep tiles here: the histogram atomics and the grid barrier would queue behind
+  // the prefetch traffic.)
   for (int i = t; i < kDigitBins; i += kSweepThreads) if (s_h[i]) atomicAdd(&hist_c[i], s_h[i]);
   grid.sync();
   stamp(st, 1);
@@ -304,7 +302,7 @@ __global__ void __launch_bounds__(kSweepThreads) k_topk_fused(const TopkArgs a) 
   constexpr int kVecIters = kTileElems / (kSweepThreads * 4);   // 4
   // Candidates collect in shared memory ACROSS tiles and go out once per CTA (a CTA sees a few hundred of them in total);
   // the staging is emptied early only when it is half full.  The first version reserved the global slots after every tile:
-  // one global atomic round trip (~1 us) with the whole CTA waiting behind it, and three barriers, per 48 KB of data.
+  // one global atomic round trip with the whole CTA waiting behind it, and three barriers, per 48 KB of data.
   auto flush_cands = [&]() {                               // uniform over the CTA; caller has synchronised
     const unsigned int nc = s_ncand < (unsigned)kSmemCand ? s_ncand : (unsigned)kSmemCand;   // slots past the staging went to global directly
     if (nc) {

@@ -1,4 +1,4 @@
-// Gradient exchange over NVLink 5 / NVSwitch peer memory (sm_100a).
+// Gradient exchange over NVLink / NVSwitch peer memory (sm_90a).
 //
 // Replaces the c10d Reducer's per-bucket  grad/W -> ncclAllReduce(SUM) -> copy-back
 // (harness_definitions/base_harness.py:81 of the reference; SURVEY K7) with ONE kernel per

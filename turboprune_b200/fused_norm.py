@@ -113,7 +113,7 @@ class _BNFn(torch.autograd.Function):
 
 
 class BatchNorm2dB200(nn.BatchNorm2d):
-    """nn.BatchNorm2d whose CUDA path is the fused sm_100a kernel; ``forward(x, residual=None, relu=False)``."""
+    """nn.BatchNorm2d whose CUDA path is the fused sm_90a kernel; ``forward(x, residual=None, relu=False)``."""
 
     def forward(self, x, residual=None, relu=False, ext_stats=None):
         """``ext_stats``: batch statistics of ``x`` already computed by the producing convolution's epilogue."""
@@ -180,7 +180,7 @@ class _MaxPoolFn(torch.autograd.Function):
 
 
 class MaxPool2dB200(nn.MaxPool2d):
-    """nn.MaxPool2d whose CUDA/NHWC path is the sm_100a kernel pair (square window, no dilation / ceil_mode)."""
+    """nn.MaxPool2d whose CUDA/NHWC path is the sm_90a kernel pair (square window, no dilation / ceil_mode)."""
 
     def forward(self, x):
         k, s, p = self.kernel_size, self.stride, self.padding

@@ -79,7 +79,8 @@ class P2PGradReducer:
     multicast address.  The switch's summation order is fixed by the fabric, not by us: replicas stay
     bit-identical (every replica receives the value rank r computed), but against the fixed rank-order sum the result
     may differ in the last bits of the LARGEST summand for W > 2 (tested: |diff| <= 4 eps * sum_r |g_r| / W); "auto" uses
-    it from 4 ranks on (281 us vs 377 us two-shot vs 331 us NCCL for ResNet-50's 102 MB on 8 GPUs; TP_P2P_NVLS=0/1 overrides).
+    it from 4 ranks on (TP_P2P_NVLS=0/1 overrides; the crossover was chosen on an earlier GPU generation and is not
+    re-measured on H100).
 
     Overlap: the masked layers / fused BN (which write their gradients straight into the bucket slots) and autograd's
     post-accumulate hooks (all other parameters) report every finished gradient through ``notify``; when the last
@@ -158,8 +159,8 @@ class P2PGradReducer:
         if numel * 4 <= (1 << 20):
             return 0
         import os
-        # measured on 8 x B200 (profiles/r02_p2p_check_8gpu.log, 102 MB bucket): in-switch 281 us, two-shot 377 us,
-        # NCCL all_reduce (NVLS) 331 us; on 2 GPUs the switch path loses (323 vs 195 us), so it starts at 4 ranks
+        # the in-switch path pays off with more ranks (on 2 GPUs two-shot was faster), so it starts at 4 ranks;
+        # TP_P2P_NVLS=0/1 overrides
         nvls = os.environ.get("TP_P2P_NVLS")
         use = (self.world >= 4) if nvls is None else (nvls == "1")
         return 2 if (has_mc and use) else 1

@@ -1,7 +1,7 @@
 """Generic train / eval loop — drop-in for the reference's ``harness_definitions/base_harness.py``.
 
 Same attributes and methods the driver relies on (``.model .train_loader .val_loader .distributed .console
-.optimizer .scheduler``; ``train_step / test_step / train_epoch / test``, reference :115-245).  B200 differences:
+.optimizer .scheduler``; ``train_step / test_step / train_epoch / test``, reference :115-245).  Differences:
   * the model is NOT wrapped in DistributedDataParallel: gradients are averaged by ``P2PGradReducer`` (one NVLink
     kernel per bucket, launched on a side stream as soon as the bucket's last gradient is written, i.e. under the
     rest of the backward pass); masks are broadcast once per pruning step, never per forward;
@@ -153,7 +153,7 @@ class BaseHarness:
         inputs, targets = batch
         inputs, targets = inputs.to(self.device, non_blocking=True), targets.to(self.device, non_blocking=True)
         if not inputs.is_cuda:
-            raise RuntimeError("turboprune_b200: the train step needs CUDA tensors (B200 / sm_100a); there is no CPU path")
+            raise RuntimeError("turboprune_b200: the train step needs CUDA tensors (H100 / sm_90a); there is no CPU path")
         sync_lr = getattr(self.optimizer, "sync_lr", None)
         key = self._graph_key(inputs, targets)
         g = self._graph if self._graph_enabled() else None

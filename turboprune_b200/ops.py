@@ -1,5 +1,5 @@
 """Torch-tensor front end of the C-ABI kernels (device memory / streams are torch's; the
-arithmetic is ours).  Every function here launches hand-written sm_100a kernels through
+arithmetic is ours).  Every function here launches hand-written sm_90a kernels through
 ``_cabi`` — there is no eager / CPU fallback.
 """
 import ctypes
@@ -123,7 +123,7 @@ def join_wgrad(device=None):
 def _require_cuda(*tensors):
     for t in tensors:
         if t is not None and not t.is_cuda:
-            raise RuntimeError("turboprune_b200 kernels need CUDA tensors (B200 / sm_100a); there is no CPU path")
+            raise RuntimeError("turboprune_b200 kernels need CUDA tensors (H100 / sm_90a); there is no CPU path")
 
 
 _ws_cache = {}

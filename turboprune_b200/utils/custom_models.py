@@ -6,7 +6,7 @@ semantics (utils/custom_models.py:18-245): layers are re-created (not copied) in
 class is looked up BY NAME in this module's namespace (``mask_layer_type`` from the config);
 ``get_overall_sparsity`` returns PERCENT; ``reset_weights`` rewinds everything except ``*mask``.
 
-B200 differences: sparsity accounting is one kernel launch + one sync instead of one ``.item()``
+Differences: sparsity accounting is one kernel launch + one sync instead of one ``.item()``
 per layer (reference :51-62), and the network is kept in channels_last so activations reach the
 masked convolutions as NHWC bf16 without a layout pass.
 """
@@ -138,7 +138,7 @@ class TorchVisionModel(PruneModel):
         if dataset in ("cifar10", "cifar100"):
             self._prepare_for_cifar(dataset)
         self._replace_layers()
-        # B200: BatchNorm / ReLU / residual-add between the masked convs run as fused NHWC kernels
+        # BatchNorm / ReLU / residual-add between the masked convs run as fused NHWC kernels
         # (same modules, parameters and state-dict keys; SURVEY.md §8(f) row 1).
         if getattr(cfg.model_params, "fuse_norm", True):
             from ..fused_norm import fuse_torchvision_blocks

@@ -20,7 +20,7 @@ def _ptr(t):
 
 def _augment(src, out_hw, r, shifts=None, flip=None, corner_y=None, corner_x=None, cut_size=0):
     if not src.is_cuda:
-        raise RuntimeError("turboprune_b200 augmentation kernels need CUDA tensors (B200 / sm_100a); there is no CPU path")
+        raise RuntimeError("turboprune_b200 augmentation kernels need CUDA tensors (H100 / sm_90a); there is no CPU path")
     lib = _cabi.load()
     src = src.contiguous().float()
     n, c = src.shape[:2]

@@ -4,7 +4,7 @@ Same class names, constructor arguments, parameter/buffer names (``weight``, ``b
 ``mask`` buffer with the weight's shape) and ``set_er_mask`` as the reference
 (utils/mask_layers.py:10-128), so checkpoints, ``custom_models.replace_layers`` and the
 ``mask_layer_type`` string lookup keep working.  What changes is ``forward``: instead of
-materialising ``mask * weight`` and calling cuDNN/cuBLAS, it launches the sm_100a
+materialising ``mask * weight`` and calling cuDNN/cuBLAS, it launches the sm_90a
 implicit-GEMM kernels (``turboprune_b200.ops``), which consume weights masked while they are
 staged to bf16 and apply the mask to the weight gradient inside wgrad.
 

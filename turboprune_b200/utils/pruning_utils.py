@@ -3,7 +3,7 @@
 Public names and call signatures are the reference's (``prune_the_model`` and the
 ``prune_<method>`` family looked up by string, utils/pruning_utils.py:23-58).  The heavy part —
 per-layer score temporaries, ``torch.cat``, single-CTA ``torch.kthvalue`` and per-layer
-``torch.where`` (:73-87, :186-203, :263-283) — is one call into the sm_100a radix-select
+``torch.where`` (:73-87, :186-203, :263-283) — is one call into the sm_90a radix-select
 kernels (``ops.topk_threshold_mask``), bit-exact with the reference's masks.
 
 Things kept on purpose:
