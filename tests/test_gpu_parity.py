@@ -912,28 +912,6 @@ def test_harness_train_epoch_vs_oracle(dev, tmp_path):
     assert abs(out["train_acc"] - acc_ref) <= 100.0 * 8 / 320                # a handful of argmax flips between two bf16 paths
 
 
-@pytest.mark.parametrize("case", [(32, 56, 64, 256, 1, 1, 0), (32, 56, 256, 64, 1, 1, 0), (40, 28, 64, 64, 3, 1, 1), (24, 28, 128, 512, 1, 1, 0)])
-def test_weight_stationary_walk_bit_identical(dev, case, monkeypatch):
-    """TP_IGEMM_WS=1 (a CTA keeps one output-channel tile's weight blocks in shared memory and streams only activation
-    tiles) computes the same dot products in the same K order: fprop and dgrad outputs bit-identical to the default walk."""
-    from turboprune_b200 import ops
-    n, hw, cin, cout, k, s_, p_ = case
-    g = torch.Generator(device=dev).manual_seed(sum(case))
-    x = torch.randn(n, cin, hw, hw, device=dev, generator=g).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
-    w = torch.randn(cout, cin, k, k, device=dev, generator=g) / (cin * k * k) ** 0.5
-    m = (torch.rand(cout, cin, k, k, device=dev, generator=g) < 0.3).float()
-    outs = {}
-    for ws in ("0", "1"):
-        monkeypatch.setenv("TP_IGEMM_WS", ws)
-        xx = x.clone().requires_grad_(True)
-        y = ops.masked_conv2d(xx, w, m, stride=(s_, s_), padding=(p_, p_))
-        gy = torch.Generator(device=dev).manual_seed(7)
-        dy = torch.randn(y.shape, device=dev, generator=gy).to(torch.bfloat16).contiguous(memory_format=torch.channels_last)
-        y.backward(dy)
-        outs[ws] = (y.detach().clone(), xx.grad.detach().clone())
-    assert torch.equal(outs["0"][0], outs["1"][0]) and torch.equal(outs["0"][1], outs["1"][1])
-
-
 # ---------------------------------------------------------------- data path (SURVEY §8(f) row 3) --------------------
 def test_cifar_augmentation_kernel_matches_reference_fixture(dev):
     """tp_cifar_augment with the draws the reference made (fixture written by running utils/dataset.py:38-98): every op

@@ -67,9 +67,8 @@ struct FwdParams {
   int out_row_pix;          // output pixels per row
   int osh, osw;
   int linear;               // output pixel index == iteration pixel index (single class, unit output stride)
-  int ws_stages, ws_b_bytes;   // weight-stationary instantiation: activation stages, bytes of the resident weight blocks
   int ldc;                  // elements between consecutive output pixels
-  int tma_store;            // 1: epilogue stages 32x64 sub-tiles in smem and stores them with TMA (tmC)
+  int staged_store;         // 1: epilogue stages 32x64 sub-tiles in smem and writes them as full 128-byte rows
   __nv_bfloat16* out;
   const float* bias;
   const __nv_bfloat16* addend;   // optional: out = acc (+ bias) + addend[pixel][channel] (same layout as out)
@@ -88,18 +87,13 @@ struct FwdParams {
 // The staging call leaves the number of empty blocks behind the last mask row: zero (any iid unstructured mask) means
 // the K loop needs no per-block test at all.
 __device__ __forceinline__ const uint32_t* live_kmask(const uint32_t* km, int words, int N) {
-#ifdef TP_NO_KMASK          // experiment builds only: compile the skip walk out
-  return nullptr;
-#else
   if (km && __ldg(km + (size_t)((N + 63) >> 6) * words) == 0u) return nullptr;
   return km;
-#endif
 }
 
 // Which K blocks of an output-channel tile hold any non-zero weight: the OR of the occupancy words of the tile's 64-row
-// groups.  Producer and MMA thread walk the K loop with one of these each and must take identical decisions: a block is
-// processed when its bit is set, or when it is the last one and nothing was processed yet (the accumulator must be
-// written at least once).
+// groups.  Producer and MMA thread walk the K loop with one of these each and must take identical decisions: both ask
+// take().
 struct KSkip {
   const uint32_t* base; int words, g0, g1; int cur_w; uint32_t bits;
   __device__ __forceinline__ void begin(const uint32_t* km, int wds, int n0, int block_n, int N) {
@@ -115,6 +109,9 @@ struct KSkip {
     }
     return (bits >> (kb & 31)) & 1u;
   }
+  // process K block kb?  Yes when its bit is set, or when it is the tile's last block (`last`) and no block was
+  // processed yet (`any`): the accumulator must be written at least once.
+  __device__ __forceinline__ bool take(int kb, bool last, bool any) { return on(kb) || (last && !any); }
 };
 
 struct WgParams {
@@ -132,15 +129,39 @@ struct WgParams {
   TapEntry taps[kMaxTaps];
 };
 
-// wgrad work item (128 output channels x nvalid 64-column chunks): true when every 64x64 block of it is empty in the
-// occupancy mask, i.e. every mask entry under it is zero (tp_stage_weights marks a block occupied as soon as one mask
-// entry is non-zero) — dW = mask * (...) is zero there whatever the activations are.
-__device__ __forceinline__ bool wg_item_empty(const uint32_t* __restrict__ km, int words, int row_groups, int m_t,
-                                              int chunk0, int nvalid) {
-  for (int r = 2 * m_t; r < 2 * m_t + 2 && r < row_groups; ++r)
-    for (int c = chunk0; c < chunk0 + nvalid; ++c)
-      if ((__ldg(km + (size_t)r * words + (c >> 5)) >> (c & 31)) & 1u) return false;
-  return true;
+// wgrad work item: split `split` (K blocks kb0 .. kb1-1) of output tile `tile` = (m_t, n_t), which covers 128 output
+// channels x the nvalid 64-column chunks from chunk0.
+struct WgItem {
+  int split, tile, m_t, n_t, chunk0, nvalid, kb0, kb1;
+  // the output-tile part (nb chunks per N tile, `chunks` in all); the finalize kernel, which knows the tile directly,
+  // uses it alone
+  __device__ __forceinline__ void set_tile(int m, int n, int m_tiles, int nb, int chunks) {
+    m_t = m; n_t = n; tile = n * m_tiles + m;
+    chunk0 = n * nb; nvalid = min(nb, chunks - chunk0);
+  }
+  // true when every 64x64 block of the tile is empty in the occupancy mask, i.e. every mask entry under it is zero
+  // (tp_stage_weights marks a block occupied as soon as one mask entry is non-zero) — dW = mask * (...) is zero there
+  // whatever the activations are.  The producer, the consumers and the finalize kernel all skip such tiles.
+  __device__ __forceinline__ bool empty(const uint32_t* __restrict__ km, int words, int Mc) const {
+    const int row_groups = (Mc + 63) >> 6;
+    for (int r = 2 * m_t; r < 2 * m_t + 2 && r < row_groups; ++r)
+      for (int c = chunk0; c < chunk0 + nvalid; ++c)
+        if ((__ldg(km + (size_t)r * words + (c >> 5)) >> (c & 31)) & 1u) return false;
+    return true;
+  }
+};
+
+// Work item -> WgItem (nb: chunks per N tile).  Split-major order: the CTAs running at the same time work on the SAME
+// pixel range for different (m, n) tiles, so each X / dY chunk comes from HBM once and from L2 for the siblings
+// (tile-major order re-reads them from HBM).
+__device__ __forceinline__ WgItem wg_item(const WgParams& p, int nb, int item) {
+  WgItem w;
+  const int ntile = p.m_tiles * p.n_tiles;
+  w.split = item / ntile;
+  const int tile = item - w.split * ntile, n_t = tile / p.m_tiles;
+  w.set_tile(tile - n_t * p.m_tiles, n_t, p.m_tiles, nb, p.chunks);
+  w.kb0 = w.split * p.kb_per_split; w.kb1 = min(p.kblocks, w.kb0 + p.kb_per_split);
+  return w;
 }
 
 __device__ __forceinline__ void decompose_pixel(int m, int P, int Q, int& n, int& p, int& q) {
@@ -175,11 +196,6 @@ __device__ __forceinline__ void fwd_mma_block(float (&acc)[BLOCK_N / 2], uint32_
 // MULTI = false: one class of output pixels (fprop, stride-1 dgrad) — the class decode, the per-row destination
 // arithmetic and the "class without taps" handling are compiled out.
 //
-// WS = true ("weight stationary", single class): when all K blocks of an output-channel tile fit in shared memory next
-// to a few activation stages (the 1x1 layers of ResNet-50's layer1-3, the 64-channel 3x3s), a CTA keeps ONE
-// output-channel tile for its whole life, loads its weight blocks once and then streams only activation tiles (the
-// dense walk re-loads BLOCK_N x 64 weights with every K block of every tile).
-//
 // BNB = true (single class, linear output): the BatchNorm backward reduction of the layer that FEEDS this convolution is
 // done here, in the dgrad epilogue, instead of by k_bn_bwd_reduce (one read of dz and one of y per such layer less, one
 // launch less): after the bf16 gradient sub-tile has been staged, each lane re-reads it row-coalesced together with the
@@ -189,13 +205,12 @@ __device__ __forceinline__ void fwd_mma_block(float (&acc)[BLOCK_N / 2], uint32_
 // The accumulators leave the registers through an fp32 exchange tile in shared memory (16-byte chunk j of row r is
 // stored at chunk j ^ (r & 7): conflict-free for both the fragment stores and the row reads), so that each epilogue lane
 // owns one output row, as the coalesced staged stores and the 32-row statistics groups need.
-template <int BLOCK_N, bool MULTI, bool WS, bool BNB>
+template <int BLOCK_N, bool MULTI, bool BNB>
 __global__ void __launch_bounds__(kThreads, 1)
 k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ FwdParams p) {
   static_assert(BLOCK_N == 64 || BLOCK_N == 128, "wgmma N of the fwd kernel");
-  static_assert(!WS || !MULTI, "weight-stationary walk: single class");
-  static_assert(!BNB || (!MULTI && !WS), "BatchNorm-backward epilogue: single class, default walk");
+  static_assert(!BNB || !MULTI, "BatchNorm-backward epilogue: single class");
   constexpr int kABytes = kBlockM * kBlockK * 2;           // 16 KB
   constexpr int kBBytes = BLOCK_N * kBlockK * 2;
   constexpr int kStageBytes = kABytes + kBBytes;
@@ -204,29 +219,19 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   pdl_trigger();
   constexpr int kStgBytes = 32 * 128;                      // one epilogue warp's 32 rows x 64 bf16 columns
-  constexpr int kMaxStages = 16;
-  const int n_stages = WS ? p.ws_stages : kStages;         // WS: a stage is the 16 KB activation tile alone
-  const int a_stride = WS ? kABytes : kStageBytes;
-  uint8_t* const a_base = WS ? smem + p.ws_b_bytes : smem; // WS: the resident weight blocks come first
-  float* const acc_tile = (float*)(a_base + n_stages * a_stride);     // 128 x BLOCK_N fp32
+  float* const acc_tile = (float*)(smem + kStages * kStageBytes);     // 128 x BLOCK_N fp32
   uint8_t* stg_base = (uint8_t*)(acc_tile + kBlockM * BLOCK_N);       // 8 warps x 4 KB (1024-B aligned)
   uint64_t* full_bar = (uint64_t*)(stg_base + 8 * kStgBytes);
-  uint64_t* empty_bar = full_bar + (WS ? kMaxStages : kStages);
-  uint64_t* bres_bar = empty_bar + (WS ? kMaxStages : kStages);       // WS: the resident weight blocks have landed
+  uint64_t* empty_bar = full_bar + kStages;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_tiles = (p.N + BLOCK_N - 1) / BLOCK_N;
   // work items: (class) x (M tile) x (N tile), classes back to back
   const int total_tiles = p.cls[p.ncls - 1].tile0 + p.cls[p.ncls - 1].m_groups * n_tiles;
-  // the w-th work item of this CTA.  WS: one fixed N tile, M tiles ws_m0, ws_m0 + ws_dm, ... (CTAs with neighbouring ids
-  // take the same M tile for the n_tiles different N tiles at about the same time: the activation tile comes from HBM once)
-  const int ws_nt = WS ? (int)blockIdx.x % n_tiles : 0;
-  const int ws_m0 = WS ? (int)blockIdx.x / n_tiles : 0, ws_dm = WS ? (int)gridDim.x / n_tiles : 1;
-  const int my_items = WS ? (p.cls[0].m_groups > ws_m0 ? (p.cls[0].m_groups - ws_m0 + ws_dm - 1) / ws_dm : 0)
-                          : (total_tiles > (int)blockIdx.x ? (total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0);
+  const int my_items = total_tiles > (int)blockIdx.x ? (total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
+  // the w-th work item of this CTA
   auto get_tile = [&](int w, int& ci, int& m_g, int& n_t) {
     ci = 0;
-    if (WS) { m_g = ws_m0 + w * ws_dm; n_t = ws_nt; return; }
     const int tile = (int)blockIdx.x + w * (int)gridDim.x;
     if (MULTI) decode_tile(p, tile, n_tiles, ci, m_g, n_t);
     else { m_g = tile / n_tiles; n_t = tile - m_g * n_tiles; }   // m-major: CTAs running together share A tiles, weights stay in L2
@@ -236,8 +241,7 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
     for (int j = 0; j < p.ncls; ++j) prefetch_tmap(&tmA.m[j]);
     prefetch_tmap(&tmB);
     // empty: one arrival per consumer warpgroup once its MMAs have read the stage
-    for (int i = 0; i < n_stages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kConsumers / 128); }
-    mbar_init(bres_bar, 1);
+    for (int i = 0; i < kStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kConsumers / 128); }
     fence_mbar_init();
   }
   __syncthreads();
@@ -248,14 +252,6 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
     if (lane == 0) {
       int stage = 0; uint32_t phase = 0;
       const uint32_t* const km = live_kmask(p.kmask, p.kmask_words, p.N);
-      if (WS && my_items > 0) {
-        // every K block of this CTA's output-channel tile, once
-        const ClsEntry& c0 = p.cls[0];
-        mbar_arrive_expect_tx(bres_bar, (uint32_t)(c0.ntaps * p.cchunks * kBBytes));
-        for (int tap = 0; tap < c0.ntaps; ++tap)
-          for (int cc = 0; cc < p.cchunks; ++cc)
-            tma_load_2d(smem + (tap * p.cchunks + cc) * kBBytes, &tmB, bres_bar, p.taps[tap].kofs + cc * kBlockK, ws_nt * BLOCK_N);
-      }
       for (int w = 0; w < my_items; ++w) {
         int ci, m_g, n_t; get_tile(w, ci, m_g, n_t);
         const ClsEntry& ce = p.cls[MULTI ? ci : 0];
@@ -266,15 +262,15 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
         const int cw = ce.base_w + cq * p.step_w, ch = ce.base_h + cp * p.step_h;
         auto load_block = [&](const TapEntry& te, int cc) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sA = a_base + stage * a_stride;
+          uint8_t* sA = smem + stage * kStageBytes;
           uint8_t* sB = sA + kABytes;
-          mbar_arrive_expect_tx(&full_bar[stage], WS ? kABytes : kStageBytes);
+          mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
           if (p.a_mode == 1)
             tma_load_im2col_4d(sA, mapA, &full_bar[stage], cc * kBlockK, cw, ch, cn, te.off_w, te.off_h);
           else
             tma_load_2d(sA, mapA, &full_bar[stage], te.kofs + cc * kBlockK, m0);
-          if (!WS) tma_load_2d(sB, &tmB, &full_bar[stage], te.kofs + cc * kBlockK, n_t * BLOCK_N);
-          if (++stage == n_stages) { stage = 0; phase ^= 1; }
+          tma_load_2d(sB, &tmB, &full_bar[stage], te.kofs + cc * kBlockK, n_t * BLOCK_N);
+          if (++stage == kStages) { stage = 0; phase ^= 1; }
         };
         const int tap_base = MULTI ? ce.tap0 : 0;     // single class: a static table offset (no dependent parameter load)
         if (!km) {
@@ -291,7 +287,7 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
             const TapEntry te = p.taps[tap_base + tap];
             for (int cc = 0; cc < p.cchunks; ++cc) {
               const bool last = tap == ce.ntaps - 1 && cc == p.cchunks - 1;
-              if (!ks.on((te.kofs >> 6) + cc) && !(last && !any)) continue;
+              if (!ks.take((te.kofs >> 6) + cc, last, any)) continue;
               any = true;
               load_block(te, cc);
             }
@@ -307,7 +303,6 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
     const int erow = quarter * 32 + lane;
     int stage = 0; uint32_t phase = 0;
     const uint32_t* const km = live_kmask(p.kmask, p.kmask_words, p.N);
-    if (WS && my_items > 0) mbar_wait(bres_bar, 0);
     // 32 fp32 accumulators of this lane's row, columns c .. c+31, from the exchange tile
     auto acc_row_ld = [&](int c, uint32_t* v) {
       const uint32_t rb = smem_u32(acc_tile) + (uint32_t)(erow * BLOCK_N * 4);
@@ -325,7 +320,7 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
       const int row = m_t * kBlockM + quarter * 32 + lane;
       const bool row_ok = row < ce.M;
       long long opix = 0;
-      if (row_ok && !p.tma_store) {       // generic output mapping, one division chain per tile
+      if (row_ok && !p.staged_store) {    // generic output mapping, one division chain per tile
         opix = row;
         if (MULTI || !p.linear) {
           int n, pp, qq; decompose_pixel(row, ce.P_it, ce.Q_it, n, pp, qq);
@@ -343,7 +338,7 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
       // the destination pixel — ONE division chain for the first row, the other seven follow by stepping 4 pixels
       long long ooff[MULTI ? 8 : 1];
       const long long rbase = (wrow0 + r_in) * ldc + c16 * 8;
-      if (MULTI && p.tma_store) {
+      if (MULTI && p.staged_store) {
         int n, pp, qq; decompose_pixel((int)(wrow0 + r_in), ce.P_it, ce.Q_it, n, pp, qq);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
@@ -357,7 +352,7 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
       if (MULTI && !has_acc) {
         // parity class no tap reaches (e.g. 3 of the 4 classes of a 1x1 stride-2 convolution): dX there is the fused addend
         // or zero — plain coalesced copies / stores; no accumulator exists, so no hand-shake with the MMA thread either
-        if (p.tma_store) {
+        if (p.staged_store) {
 #pragma unroll 1
           for (int c = half * 64; c < BLOCK_N; c += 128) {
             const int n0 = n_t * BLOCK_N + c;
@@ -385,17 +380,16 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
 #pragma unroll
         for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
         int prev = -1;                        // stage of the previous K block: freed once its MMAs have completed
-        auto mma_block = [&](uint32_t accumulate, int kb) {
+        auto mma_block = [&](uint32_t accumulate) {
           mbar_wait(&full_bar[stage], phase);
-          const uint32_t s_addr = smem_u32(a_base + stage * a_stride);
-          const uint32_t b_addr = WS ? smem_u32(smem + kb * kBBytes) : s_addr + kABytes;   // WS: K block kb of the resident tile
+          const uint32_t s_addr = smem_u32(smem + stage * kStageBytes);
           wgmma_fence();
-          fwd_mma_block<BLOCK_N>(acc, s_addr + (uint32_t)(wg * (kABytes / 2)), b_addr, accumulate);
+          fwd_mma_block<BLOCK_N>(acc, s_addr + (uint32_t)(wg * (kABytes / 2)), s_addr + kABytes, accumulate);
           wgmma_commit();
           wgmma_wait<1>();
           if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
           prev = stage;
-          if (++stage == n_stages) { stage = 0; phase ^= 1; }
+          if (++stage == kStages) { stage = 0; phase ^= 1; }
         };
         // one walk with a single MMA call site (two would make ptxas serialise the wgmma pipeline)
         KSkip ks; uint32_t any = 0;
@@ -404,8 +398,8 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
           const int kb0 = p.taps[(MULTI ? ce.tap0 : 0) + tap].kofs >> 6;
           for (int cc = 0; cc < p.cchunks; ++cc) {
             const bool last = tap == ce.ntaps - 1 && cc == p.cchunks - 1;
-            if (km && !ks.on(kb0 + cc) && !(last && !any)) continue;           // same decision as the producer
-            mma_block(any, tap * p.cchunks + cc);
+            if (km && !ks.take(kb0 + cc, last, any)) continue;
+            mma_block(any);
             any = 1;
           }
         }
@@ -425,7 +419,7 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
           }
         bar_sync(1, kConsumers);
       }
-      if (p.tma_store) {
+      if (p.staged_store) {
         // accumulators -> registers -> 128B-swizzled smem sub-tile (32 rows x 64 cols) -> coalesced global
         // stores, so every output line leaves the SM as full 128-byte rows instead of 32 scattered 16-byte pieces.
         // Everything that does not depend on the column chunk is hoisted (row pointers, validity, swizzled
@@ -434,7 +428,6 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
         const uint32_t buf = smem_u32(stg_base + warp * kStgBytes);
         __nv_bfloat16* const gout = p.out;
         const __nv_bfloat16* const gadd = p.addend;
-        {
         const float* bias = p.bias;
         float* stats = p.stats ? p.stats + (long long)(m_t * 4 + quarter) * 2 * N + c16 * 8 : nullptr;
         const uint32_t wr_base = buf + lane * 128;                              // my row in the staging tile
@@ -506,15 +499,21 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
           uint4 o[8];
 #pragma unroll
           for (int i = 0; i < 8; ++i) o[i] = lds128(((i & 1) ? rd_odd : rd_even) + (uint32_t)((i >> 1) * 1024));
+          // per-channel sums of the row-coalesced view: this lane owns channels n0 + c16*8 .. +8 of rows r_in + 4i.
+          // BNB: sum g and sum g * xhat of the gradient, gated before it is stored; otherwise (stats) the BatchNorm batch statistics sum o and
+          // sum o^2 of exactly the values stored (bf16-rounded).  A fixed-order xor tree over the 4 row groups finishes
+          // the 32 rows.
+          float s1[8], s2[8];
+#pragma unroll
+          for (int q = 0; q < 8; ++q) { s1[q] = 0.f; s2[q] = 0.f; }
           if (BNB) {
-            // gate + BatchNorm backward sums on the row-coalesced view: this lane owns channels n0 + c16*8 .. +8 of rows r_in + 4i
             uint4 yv[8];
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
               yv[i] = make_uint4(0u, 0u, 0u, 0u);
               if (i * 4 + r_in < rows_left && col_ok) yv[i] = *reinterpret_cast<const uint4*>(p.bn_y + row_off(i) + n0);
             }
-            float sc[8], sf[8], is_[8], nm[8], s1[8], s2[8];
+            float sc[8], sf[8], is_[8], nm[8];
             if (col_ok) {
               const int cb = n0 + c16 * 8;
 #pragma unroll
@@ -535,8 +534,6 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
               for (int q = 0; q < 8; ++q) { sc[q] = 0.f; sf[q] = 0.f; is_[q] = 0.f; nm[q] = 0.f; }
             }
 #pragma unroll
-            for (int q = 0; q < 8; ++q) { s1[q] = 0.f; s2[q] = 0.f; }
-#pragma unroll
             for (int i = 0; i < 8; ++i) {
               if (i * 4 + r_in < rows_left) {
                 __nv_bfloat162* gh = reinterpret_cast<__nv_bfloat162*>(&o[i]);
@@ -554,30 +551,11 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
                 }
               }
             }
-#pragma unroll
-            for (int i = 0; i < 8; ++i)
-              if (i * 4 + r_in < rows_left && col_ok) *reinterpret_cast<uint4*>(gout + row_off(i) + n0) = o[i];
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              s1[q] += __shfl_xor_sync(0xffffffffu, s1[q], 8);  s2[q] += __shfl_xor_sync(0xffffffffu, s2[q], 8);
-              s1[q] += __shfl_xor_sync(0xffffffffu, s1[q], 16); s2[q] += __shfl_xor_sync(0xffffffffu, s2[q], 16);
-            }
-            if (r_in == 0 && col_ok) {
-              float4* d1 = reinterpret_cast<float4*>(stats + n0);
-              float4* d2 = reinterpret_cast<float4*>(stats + N + n0);
-              d1[0] = make_float4(s1[0], s1[1], s1[2], s1[3]); d1[1] = make_float4(s1[4], s1[5], s1[6], s1[7]);
-              d2[0] = make_float4(s2[0], s2[1], s2[2], s2[3]); d2[1] = make_float4(s2[4], s2[5], s2[6], s2[7]);
-            }
-          } else {
+          }
 #pragma unroll
           for (int i = 0; i < 8; ++i)
             if (i * 4 + r_in < rows_left && col_ok) *reinterpret_cast<uint4*>(gout + row_off(i) + n0) = o[i];
-          if (stats) {
-            // BatchNorm batch statistics of exactly the values just stored (bf16-rounded): this thread owns 8 channels
-            // of rows r_in, r_in+4, ...; a fixed-order xor tree over the 4 row groups finishes the 32 rows
-            float s1[8], s2[8];
-#pragma unroll
-            for (int q = 0; q < 8; ++q) { s1[q] = 0.f; s2[q] = 0.f; }
+          if (!BNB && stats) {       // after the stores, so that they leave while the sums are computed
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
               if (i * 4 + r_in < rows_left) {
@@ -590,6 +568,8 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
                 }
               }
             }
+          }
+          if (BNB || stats) {
 #pragma unroll
             for (int q = 0; q < 8; ++q) {
               s1[q] += __shfl_xor_sync(0xffffffffu, s1[q], 8);  s2[q] += __shfl_xor_sync(0xffffffffu, s2[q], 8);
@@ -602,10 +582,8 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
               d2[0] = make_float4(s2[0], s2[1], s2[2], s2[3]); d2[1] = make_float4(s2[4], s2[5], s2[6], s2[7]);
             }
           }
-          }   // !BNB
           __syncwarp();
         }
-        }   // has_acc
       } else {
 #pragma unroll 1
       for (int c = half * 32; c < BLOCK_N; c += 64) {
@@ -685,7 +663,6 @@ k_igemm_wgrad(const __grid_constant__ CUtensorMap tmA /* dY [Kpix, Cout] */,
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int items = p.m_tiles * p.n_tiles * p.splits;
   constexpr int ncols = NB * 64;
-  const int row_groups = (p.Mc + 63) >> 6;
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmA); prefetch_tmap(&tmB);
@@ -700,17 +677,9 @@ k_igemm_wgrad(const __grid_constant__ CUtensorMap tmA /* dY [Kpix, Cout] */,
     if (lane == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int item = blockIdx.x; item < items; item += gridDim.x) {
-        // split-major order: the CTAs running at the same time work on the SAME pixel range for different
-        // (m, n) tiles, so each X / dY chunk comes from HBM once and from L2 for the siblings (tile-major order
-        // re-reads them from HBM)
-        const int ntile = p.m_tiles * p.n_tiles;
-        const int split = item / ntile, tile = item - split * ntile;
-        const int n_t = tile / p.m_tiles, m_t = tile % p.m_tiles;
-        const int kb0 = split * p.kb_per_split;
-        const int kb1 = min(p.kblocks, kb0 + p.kb_per_split);
-        const int chunk0 = n_t * NB;
-        const int nvalid = min(NB, p.chunks - chunk0);
-        if (km && wg_item_empty(km, p.kmask_words, row_groups, m_t, chunk0, nvalid)) continue;   // all three roles skip the same items
+        const WgItem it = wg_item(p, NB, item);
+        if (km && it.empty(km, p.kmask_words, p.Mc)) continue;
+        const int m_t = it.m_t, chunk0 = it.chunk0, nvalid = it.nvalid, kb0 = it.kb0, kb1 = it.kb1;
         // Everything that needs an integer division is hoisted out of the K loop (one producer thread
         // feeds the whole SM): per-chunk (tap, channel) coordinates once per item, and the pixel
         // coordinate of a K block advanced incrementally by 64 = sn*P*Q + sp*Q + sq.
@@ -752,14 +721,9 @@ k_igemm_wgrad(const __grid_constant__ CUtensorMap tmA /* dY [Kpix, Cout] */,
     const int wg = warp >> 2;                 // rows (output channels) 64*wg .. 64*wg+63 of the tile
     int stage = 0; uint32_t phase = 0;
     for (int item = blockIdx.x; item < items; item += gridDim.x) {
-      const int ntile = p.m_tiles * p.n_tiles;
-      const int split = item / ntile, tile = item - split * ntile;
-      if (km) {
-        const int n_t = tile / p.m_tiles, m_t = tile - n_t * p.m_tiles;
-        if (wg_item_empty(km, p.kmask_words, row_groups, m_t, n_t * NB, min(NB, p.chunks - n_t * NB))) continue;
-      }
-      const int kb0 = split * p.kb_per_split;
-      const int kb1 = min(p.kblocks, kb0 + p.kb_per_split);
+      const WgItem it = wg_item(p, NB, item);
+      if (km && it.empty(km, p.kmask_words, p.Mc)) continue;
+      const int kb0 = it.kb0, kb1 = it.kb1;
       float acc[NB * 32];
 #pragma unroll
       for (int i = 0; i < NB * 32; ++i) acc[i] = 0.f;
@@ -779,7 +743,7 @@ k_igemm_wgrad(const __grid_constant__ CUtensorMap tmA /* dY [Kpix, Cout] */,
       acc_fence(acc);
       if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
       // fragments -> fp32 partial tile [128][ncols]: 4 lanes write 32 contiguous bytes of a row
-      float* ptile = p.partial + ((long long)tile * p.splits + split) * kBlockM * ncols;
+      float* ptile = p.partial + ((long long)it.tile * p.splits + it.split) * kBlockM * ncols;
       const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
       for (int j = 0; j < ncols / 8; ++j)
@@ -798,13 +762,13 @@ k_igemm_wgrad(const __grid_constant__ CUtensorMap tmA /* dY [Kpix, Cout] */,
 // CTA per channel: 18 dependent rounds of L2/DRAM latency for a 3x3x64 layer.)
 __global__ void __launch_bounds__(256) k_wgrad_finalize(const float* __restrict__ partial, const float* __restrict__ mask,
                                                         float* __restrict__ dw, int cout, int cin_real, int cin_p, int rs,
-                                                        int nb, int m_tiles, int n_tiles, int splits, int sl,
+                                                        int nb, int m_tiles, int splits, int sl,
                                                         const uint32_t* __restrict__ kmask, int kmask_words) {
   pdl_enter();
   __shared__ float s_lane[256];
   const uint32_t* const km = live_kmask(kmask, kmask_words, cout);
   const int co = blockIdx.x;
-  const int m_t = co / kBlockM, r = co % kBlockM;
+  const int r = co % kBlockM;
   const int ktot = rs * cin_p;
   const int ncols = nb * 64;
   const int KT = 256 / sl;
@@ -813,21 +777,23 @@ __global__ void __launch_bounds__(256) k_wgrad_finalize(const float* __restrict_
   const long long sstride = (long long)kBlockM * ncols;          // floats between consecutive splits of a tile
   float a[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   // a work item the GEMM skipped has no partials (the workspace holds whatever was there): its gradient is exactly zero
-  const int chunks = (ktot + 63) >> 6;
-  const bool skipped = km && kk < ktot &&
-                       wg_item_empty(km, kmask_words, (cout + 63) >> 6, m_t, ((kk >> 6) / nb) * nb, min(nb, chunks - ((kk >> 6) / nb) * nb));
-  if (kk < ktot && !skipped) {
-    const int chunk = kk >> 6, n_t = chunk / nb, col = (chunk - n_t * nb) * 64 + (kk & 63);
-    const float* base = partial + ((((long long)n_t * m_tiles + m_t) * splits) * kBlockM + r) * ncols + col;
-    int sp = sj;
-    for (; sp + 7 * sl < splits; sp += 8 * sl) {
-      float v[8];
+  bool skipped = false;
+  if (kk < ktot) {
+    const int chunk = kk >> 6;
+    WgItem it; it.set_tile(co / kBlockM, chunk / nb, m_tiles, nb, (ktot + 63) >> 6);     // the tile holding (co, kk)
+    skipped = km && it.empty(km, kmask_words, cout);
+    if (!skipped) {
+      const float* base = partial + (((long long)it.tile * splits) * kBlockM + r) * ncols + (chunk - it.chunk0) * 64 + (kk & 63);
+      int sp = sj;
+      for (; sp + 7 * sl < splits; sp += 8 * sl) {
+        float v[8];
 #pragma unroll
-      for (int j = 0; j < 8; ++j) v[j] = __ldcs(base + (long long)(sp + j * sl) * sstride);
+        for (int j = 0; j < 8; ++j) v[j] = __ldcs(base + (long long)(sp + j * sl) * sstride);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) a[j] += v[j];
+        for (int j = 0; j < 8; ++j) a[j] += v[j];
+      }
+      for (; sp < splits; sp += sl) a[0] += __ldcs(base + (long long)sp * sstride);
     }
-    for (; sp < splits; sp += sl) a[0] += __ldcs(base + (long long)sp * sstride);
   }
   s_lane[sj * KT + kl] = ((a[0] + a[1]) + (a[2] + a[3])) + ((a[4] + a[5]) + (a[6] + a[7]));
   __syncthreads();
@@ -978,15 +944,34 @@ static int make_im2col_map(CUtensorMap* m, const void* ptr, int n, int h, int w,
   return TP_OK;
 }
 
+// Geometry of a layer's wgrad GEMM: output tiles of 128 channels x nb 64-column chunks of K = (tap, cin), 64-pixel K
+// blocks, and the largest split count pick_wgrad_splits() may choose.  The workspace size and the launch both derive
+// from this one definition.
+struct WgGeom {
+  int chunks, nb, m_tiles, n_tiles, kblocks, smax;
+  size_t partial_bytes(int splits) const { return (size_t)m_tiles * n_tiles * splits * kBlockM * nb * 64 * sizeof(float); }
+};
+
+static WgGeom wgrad_geom(const tp_conv_desc* d) {
+  WgGeom g;
+  g.chunks = (d->r * d->s * d->cin + 63) / 64;
+  g.nb = g.chunks >= 4 ? 4 : g.chunks;
+  g.m_tiles = (d->cout + kBlockM - 1) / kBlockM;
+  g.n_tiles = (g.chunks + g.nb - 1) / g.nb;
+  g.kblocks = (int)(((long long)d->n * d->p * d->q + 63) / 64);
+  g.smax = (2 * sm_count()) / (g.m_tiles * g.n_tiles);
+  if (g.smax > g.kblocks) g.smax = g.kblocks;
+  if (g.smax < 1) g.smax = 1;
+  return g;
+}
+
 // Split-K factor of the wgrad GEMM.  Every (tile, split) item costs its share of the K loop plus a fixed 128 x nb*64
 // fp32 partial tile (written once, read once by the finalize pass), so the cheapest choice is the SMALLEST split
 // count that reaches the minimal makespan over the persistent CTAs — not "as many as fit in two waves": at a per-GPU
 // batch of 64 the partial tiles were most of the wgrad traffic (54 layers x ~300 items x 128 KB, twice).
-static int pick_wgrad_splits(int tiles, int kblocks, int nb) {
+static int pick_wgrad_splits(const WgGeom& g) {
   const int sms = sm_count();
-  int smax = (2 * sms) / tiles;
-  if (smax > kblocks) smax = kblocks;
-  if (smax < 1) smax = 1;
+  const int tiles = g.m_tiles * g.n_tiles, kblocks = g.kblocks, nb = g.nb;
   // Relative costs (only their ratios decide): a 64-pixel K block (48 KB of operands, one 128 x nb*64 x 64 MMA group),
   // storing one partial tile from the accumulator registers to global, and the finalize traffic of one partial tile.
   // These weights were calibrated on an earlier GPU generation (where the partial tile was drained through tensor memory)
@@ -997,7 +982,7 @@ static int pick_wgrad_splits(int tiles, int kblocks, int nb) {
   const double c_part = 0.33 * nb;
   const double c_fin = 0.013 * nb;
   int best = 1; double best_cost = 1e30;
-  for (int s = 1; s <= smax; ++s) {
+  for (int s = 1; s <= g.smax; ++s) {
     const int kb = (kblocks + s - 1) / s;
     const int s_eff = (kblocks + kb - 1) / kb;      // no empty splits
     const long long items = (long long)tiles * s_eff;
@@ -1012,15 +997,20 @@ static bool is_plain_gemm(const tp_conv_desc* d) {
   return d->r == 1 && d->s == 1 && d->stride_h == 1 && d->stride_w == 1 && d->pad_h == 0 && d->pad_w == 0;
 }
 
+// tap table of a single-class walk over an R x S filter whose K axis is (r, s, c) with c < cin: tap (r, s) gathers at
+// im2col offset (s, r) and starts at K column (r*S + s) * cin
+static void fill_taps(TapEntry* taps, int R, int S, int cin) {
+  for (int r = 0; r < R; ++r) for (int s = 0; s < S; ++s) {
+    TapEntry& t = taps[r * S + s];
+    t.off_w = (uint16_t)s; t.off_h = (uint16_t)r; t.kofs = (r * S + s) * cin;
+  }
+}
+
 static int pick_block_n(long long m_tiles, int n) {
   // favour wide tiles (fewer re-reads of the activation tile), but keep the last wave full.  128 is the widest tile:
   // a warpgroup holds its 64 x BLOCK_N fp32 accumulators in registers, and the 128 x BLOCK_N exchange tile plus four
   // 32 KB stages fill the 227 KB of shared memory.
   const int sms = sm_count();
-  if (const char* e = getenv("TP_IGEMM_BN")) {        // experiments only: force the tile width
-    const int f = atoi(e);
-    if ((f == 64 || f == 128) && (f == 64 || n > f / 2)) return f;
-  }
   int best = 64; double best_score = -1;
   const int cands[2] = {128, 64};
   const double weight[2] = {1.0, 0.82};
@@ -1036,25 +1026,15 @@ static int pick_block_n(long long m_tiles, int n) {
 }
 
 constexpr int kSmemMax = 232448;                 // 227 KB: the per-CTA opt-in limit of sm_90
-constexpr int kWsMinStages = 3;                  // activation stages the weight-stationary walk keeps in flight at least
 
-template <int BN, bool MULTI, bool WS, bool BNB = false>
+template <int BN, bool MULTI, bool BNB = false>
 static int launch_fwd(const AMaps& a, const CUtensorMap& b, FwdParams& p, cudaStream_t st) {
-  constexpr int kStages = fwd_stages(BN);
-  constexpr int kTail = fwd_tail(BN);
-  int smem = kStages * (kBlockM * kBlockK * 2 + BN * kBlockK * 2) + kTail;
-  static_assert(fwd_stages(BN) * (kBlockM * kBlockK * 2 + BN * kBlockK * 2) + fwd_tail(BN) <= kSmemMax, "fwd smem budget");
+  constexpr int smem = fwd_stages(BN) * (kBlockM * kBlockK * 2 + BN * kBlockK * 2) + fwd_tail(BN);
+  static_assert(smem <= kSmemMax, "fwd smem budget");
   const int n_tiles = (p.N + BN - 1) / BN;
-  if (WS) {
-    p.ws_b_bytes = p.cls[0].ntaps * p.cchunks * BN * kBlockK * 2;
-    p.ws_stages = (kSmemMax - kTail - p.ws_b_bytes) / (kBlockM * kBlockK * 2);
-    if (p.ws_stages > 16) p.ws_stages = 16;
-    if (p.ws_stages < kWsMinStages) return TP_ERR_UNSUPPORTED;
-    smem = p.ws_b_bytes + p.ws_stages * kBlockM * kBlockK * 2 + kTail;
-  }
   static bool attr_set = false;
   if (!attr_set) {
-    TP_CUDA_CHECK(cudaFuncSetAttribute(k_igemm_fwd<BN, MULTI, WS, BNB>, cudaFuncAttributeMaxDynamicSharedMemorySize, WS ? kSmemMax : smem));
+    TP_CUDA_CHECK(cudaFuncSetAttribute(k_igemm_fwd<BN, MULTI, BNB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_set = true;
   }
   // work items: per class, (M tiles) x (N tiles), classes back to back
@@ -1066,9 +1046,8 @@ static int launch_fwd(const AMaps& a, const CUtensorMap& b, FwdParams& p, cudaSt
     ctiles += (long long)p.cls[c].m_groups * n_tiles;
   }
   if (ctiles > 0x7fffffffll || ctiles <= 0) return TP_ERR_UNSUPPORTED;
-  int grid = (int)(ctiles < sm_count() ? ctiles : sm_count());
-  if (WS) grid = (sm_count() / n_tiles) * n_tiles;           // every CTA owns one N tile: a whole number of CTAs per N tile
-  TP_CUDA_CHECK(launch(k_igemm_fwd<BN, MULTI, WS, BNB>, dim3(grid), dim3(kThreads), (size_t)smem, st, a, b, p));
+  const int grid = (int)(ctiles < sm_count() ? ctiles : sm_count());
+  TP_CUDA_CHECK(launch(k_igemm_fwd<BN, MULTI, BNB>, dim3(grid), dim3(kThreads), (size_t)smem, st, a, b, p));
   TP_LAUNCH_CHECK();
   return TP_OK;
 }
@@ -1078,36 +1057,23 @@ static int run_fwd(const AMaps& a, const CUtensorMap& b, FwdParams& p, int bn, c
   // (for any pixel mapping: a strided dgrad's parity classes compute the destination pixel of each row)
   p.linear = p.ncls == 1 && p.osh == 1 && p.osw == 1 && p.cls[0].oah == 0 && p.cls[0].oaw == 0 &&
              p.out_row_pix == p.cls[0].Q_it && p.out_img_pix == (long long)p.cls[0].P_it * p.cls[0].Q_it;
-  p.tma_store = (p.ldc % 8 == 0 && p.N % 8 == 0 && (((uintptr_t)p.out) & 15) == 0 &&
-                 (!p.addend || (((uintptr_t)p.addend) & 15) == 0)) ? 1 : 0;
-  if (p.stats && !(p.tma_store && p.linear)) return TP_ERR_UNSUPPORTED;
+  p.staged_store = (p.ldc % 8 == 0 && p.N % 8 == 0 && (((uintptr_t)p.out) & 15) == 0 &&
+                    (!p.addend || (((uintptr_t)p.addend) & 15) == 0)) ? 1 : 0;
+  if (p.stats && !(p.staged_store && p.linear)) return TP_ERR_UNSUPPORTED;
   // the general-mapping instantiation only where it is needed: parity classes, or a single class whose output is not
   // the iteration order itself
   const bool multi = !p.linear;
   if (multi) {
-    if (bn == 128) return launch_fwd<128, true, false>(a, b, p, st);
-    return launch_fwd<64, true, false>(a, b, p, st);
+    if (bn == 128) return launch_fwd<128, true>(a, b, p, st);
+    return launch_fwd<64, true>(a, b, p, st);
   }
   if (p.bn_y) {      // BatchNorm-backward epilogue (needs the linear staged path; the caller checked the shapes)
-    if (!p.tma_store || !p.stats) return TP_ERR_UNSUPPORTED;
-    if (bn == 128) return launch_fwd<128, false, false, true>(a, b, p, st);
-    return launch_fwd<64, false, false, true>(a, b, p, st);
-  }
-  // weight-stationary walk: the tile's weight blocks fit next to >= 3 activation stages, there is a whole number of CTAs
-  // per N tile and enough M tiles for every CTA to amortise the one-time weight load.  Opt-in (TP_IGEMM_WS=1),
-  // parity-tested against the default walk.
-  const int n_tiles = (p.N + bn - 1) / bn;
-  const long long m_tiles = (p.cls[0].M + kBlockM - 1) / kBlockM;
-  const long long b_bytes = (long long)p.cls[0].ntaps * p.cchunks * bn * kBlockK * 2;
-  const long long ws_max_b = (long long)kSmemMax - (bn == 128 ? fwd_tail(128) : fwd_tail(64)) - kWsMinStages * kBlockM * kBlockK * 2;
-  const char* e = getenv("TP_IGEMM_WS");
-  const bool ws = e && atoi(e) != 0 && b_bytes <= ws_max_b && n_tiles <= sm_count() / 2 && m_tiles >= 4ll * (sm_count() / n_tiles);
-  if (ws) {
+    if (!p.staged_store || !p.stats) return TP_ERR_UNSUPPORTED;
     if (bn == 128) return launch_fwd<128, false, true>(a, b, p, st);
     return launch_fwd<64, false, true>(a, b, p, st);
   }
-  if (bn == 128) return launch_fwd<128, false, false>(a, b, p, st);
-  return launch_fwd<64, false, false>(a, b, p, st);
+  if (bn == 128) return launch_fwd<128, false>(a, b, p, st);
+  return launch_fwd<64, false>(a, b, p, st);
 }
 
 template <int NB>
@@ -1132,20 +1098,9 @@ extern "C" {
 size_t tp_conv_workspace_bytes(const tp_conv_desc* d, int op) {
   if (!d) return 0;
   if (op != 2) return 256;
-  // wgrad: split-K partial tiles
-  const int cin_p = d->cin;
-  const int ktot = ((d->r * d->s * cin_p) + 63) / 64 * 64;
-  const int chunks = ktot / 64;
-  const int nb = chunks >= 4 ? 4 : chunks;
-  const int m_tiles = (d->cout + kBlockM - 1) / kBlockM;
-  const int n_tiles = (chunks + nb - 1) / nb;
-  const long long kpix = (long long)d->n * d->p * d->q;
-  const int kblocks = (int)((kpix + 63) / 64);
-  const int sms = sm_count();
-  int splits = (2 * sms) / (m_tiles * n_tiles);          // upper bound of pick_wgrad_splits()
-  if (splits > kblocks) splits = kblocks;
-  if (splits < 1) splits = 1;
-  return (size_t)m_tiles * n_tiles * splits * kBlockM * nb * 64 * sizeof(float) + 1024;
+  // wgrad: split-K partial tiles at the largest split count pick_wgrad_splits() may choose
+  const WgGeom g = wgrad_geom(d);
+  return g.partial_bytes(g.smax) + 1024;
 }
 
 size_t tp_conv_stats_rows(const tp_conv_desc* d) {
@@ -1180,10 +1135,7 @@ int tp_conv_fprop_stats(const tp_conv_desc* d, const void* x, const void* wf, co
   p.ldc = d->cout; p.out = (__nv_bfloat16*)y; p.bias = (const float*)bias_f32;
   p.stats = (float*)stats;
   p.kmask = (const uint32_t*)kmask_f; p.kmask_words = (int)tp_kblock_mask_words((int64_t)d->r * d->s * d->cin);
-  for (int r = 0; r < d->r; ++r) for (int s = 0; s < d->s; ++s) {
-    TapEntry& t = p.taps[r * d->s + s];
-    t.off_w = (uint16_t)s; t.off_h = (uint16_t)r; t.kofs = (r * d->s + s) * d->cin;
-  }
+  fill_taps(p.taps, d->r, d->s, d->cin);
   AMaps ta; CUtensorMap tb;
   if (is_plain_gemm(d)) {
     p.a_mode = 0;
@@ -1260,10 +1212,7 @@ static int conv_dgrad_impl(const tp_conv_desc* d, const void* dy, const void* wd
     p.ncls = 1; p.osh = 1; p.osw = 1;
     ClsEntry& ce = p.cls[0];
     ce.M = p.M; ce.P_it = d->h; ce.Q_it = d->w; ce.ntaps = R * S; ce.tap0 = 0; ce.oah = 0; ce.oaw = 0;
-    for (int r = 0; r < R; ++r) for (int s = 0; s < S; ++s) {
-      TapEntry& t = p.taps[r * S + s];
-      t.off_w = (uint16_t)s; t.off_h = (uint16_t)r; t.kofs = (r * S + s) * cop;
-    }
+    fill_taps(p.taps, R, S, cop);
     if (is_plain_gemm(d)) {
       p.a_mode = 0;
       rc = make_tiled_map(&ta.m[0], dy, (uint64_t)cop, (uint64_t)p.M, (uint64_t)cop, kBlockM); if (rc) return rc;
@@ -1332,26 +1281,22 @@ int tp_conv_wgrad(const tp_conv_desc* d, const void* x, const void* dy, const vo
   p.Mc = d->cout;
   p.Kpix = d->n * d->p * d->q;
   p.P_it = d->p; p.Q_it = d->q;
-  const int ktot = (rs * d->cin + 63) / 64 * 64;
-  p.chunks = ktot / 64;
+  const WgGeom g = wgrad_geom(d);
+  p.chunks = g.chunks;
   p.cchunks = (d->cin + 63) / 64;
-  p.nb = p.chunks >= 4 ? 4 : p.chunks;
-  p.m_tiles = (d->cout + kBlockM - 1) / kBlockM;
-  p.n_tiles = (p.chunks + p.nb - 1) / p.nb;
-  p.kblocks = (p.Kpix + 63) / 64;
+  p.nb = g.nb;
+  p.m_tiles = g.m_tiles;
+  p.n_tiles = g.n_tiles;
+  p.kblocks = g.kblocks;
   const int sms = sm_count();
-  int splits = pick_wgrad_splits(p.m_tiles * p.n_tiles, p.kblocks, p.nb);
+  int splits = pick_wgrad_splits(g);
   p.kb_per_split = (p.kblocks + splits - 1) / splits;
   splits = (p.kblocks + p.kb_per_split - 1) / p.kb_per_split;     // no empty splits
   p.splits = splits;
-  const size_t need = (size_t)p.m_tiles * p.n_tiles * splits * kBlockM * p.nb * 64 * sizeof(float);
-  if (ws_bytes < need) return TP_ERR_WORKSPACE;
+  if (ws_bytes < g.partial_bytes(splits)) return TP_ERR_WORKSPACE;
   p.partial = (float*)ws;
   p.kmask = (const uint32_t*)kmask_f; p.kmask_words = (int)tp_kblock_mask_words((int64_t)rs * d->cin);
-  for (int r = 0; r < d->r; ++r) for (int s = 0; s < d->s; ++s) {
-    TapEntry& t = p.taps[r * d->s + s];
-    t.off_w = (uint16_t)s; t.off_h = (uint16_t)r; t.kofs = (r * d->s + s) * d->cin;
-  }
+  fill_taps(p.taps, d->r, d->s, d->cin);
   CUtensorMap ta, tb;
   rc = make_tiled_map(&ta, dy, (uint64_t)d->cout, (uint64_t)p.Kpix, (uint64_t)d->cout, 64); if (rc) return rc;
   if (is_plain_gemm(d)) {
@@ -1375,8 +1320,8 @@ int tp_conv_wgrad(const tp_conv_desc* d, const void* x, const void* dy, const vo
   // split lanes only pay when there are many splits (skinny layers); wide-K layers keep all 256 threads on K
   const int sl = splits >= 64 ? 8 : (splits >= 32 ? 4 : (splits >= 16 ? 2 : 1));
   const int fin_kt = 256 / sl;
-  launch(k_wgrad_finalize, dim3(d->cout, (rs * d->cin + fin_kt - 1) / fin_kt), 256, 0, st, 
-      p.partial, (const float*)mask, (float*)dw, d->cout, cin_real, d->cin, rs, p.nb, p.m_tiles, p.n_tiles, splits, sl,
+  launch(k_wgrad_finalize, dim3(d->cout, (rs * d->cin + fin_kt - 1) / fin_kt), 256, 0, st,
+      p.partial, (const float*)mask, (float*)dw, d->cout, cin_real, d->cin, rs, p.nb, p.m_tiles, splits, sl,
       p.kmask, p.kmask_words);
   TP_LAUNCH_CHECK();
   if (db) {

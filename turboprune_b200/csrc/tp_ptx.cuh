@@ -74,16 +74,6 @@ __device__ __forceinline__ void tma_load_im2col_4d(void* dst, const CUtensorMap*
       : "memory");
 }
 
-// smem -> global tile store (coalesced full lines; clips at the tensor bounds)
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-               :: "l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" :: "n"(N) : "memory"); }
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
 // ---- wgmma ---------------------------------------------------------------------------------
 // Shared-memory matrix descriptor (sm_90 GMMA layout): start address, leading- and stride-dimension byte offsets in
 // 16-byte units, layout type in [62,64) (1 = 128-byte swizzle).
