@@ -6,10 +6,16 @@
 // appears here as a separate pass: fprop/dgrad consume bf16 weights that were masked while
 // being staged (tp_stage_weights), wgrad applies the mask in its finalize step.
 //
-// Two persistent, warp-specialised kernels (1 CTA / SM, 288 threads):
-//   warps 0..7 : two consumer warpgroups; warpgroup g issues the wgmma of rows 64g .. 64g+63 of the 128-row tile,
-//                then all eight warps run the epilogue
-//   warp 8     : TMA producer (one elected lane); runs ahead into the next tile while the epilogue drains
+// Two persistent, warp-specialised kernels (1 CTA / SM):
+//   k_igemm_fwd (384 threads, ping-pong consumers):
+//     warpgroup 0    : TMA producer (one lane; the warpgroup gives its registers up to the consumers)
+//     warpgroups 1, 2: consumers; the CTA's work items alternate between them and each owns its whole 128 x BLOCK_N
+//                      tile (MMA and epilogue).  Their mainloops take turns, so one warpgroup's epilogue runs under
+//                      the other's MMAs and the tensor cores do not wait for the epilogue.
+//   k_igemm_wgrad (288 threads):
+//     warps 0..7     : two consumer warpgroups; warpgroup g issues the wgmma of rows 64g .. 64g+63 of the 128-row
+//                      tile, then stores its fragments (the K loops are long, the epilogue is one store)
+//     warp 8         : TMA producer (one elected lane)
 //
 //   k_igemm_fwd  : D[pixels, Cout] = A[pixels, K] * W[Cout, K]^T          (fprop, dgrad)
 //                  A tile 128 pixels x 64 channels by TMA im2col (any r,s,stride,pad) or by
@@ -29,15 +35,28 @@ using namespace ptx;
 constexpr int kBlockM = 128;         // two wgmma M = 64 halves
 constexpr int kBlockK = 64;          // 64 bf16 = 128 B = one swizzle row
 constexpr int kConsumers = 256;      // two consumer warpgroups
-constexpr int kThreads = kConsumers + 32;   // + the TMA producer warp (both kernels)
+constexpr int kThreads = kConsumers + 32;   // k_igemm_wgrad: + the TMA producer warp
 constexpr int kProducerWarp = kConsumers / 32;
+constexpr int kFwdThreads = 3 * 128;        // k_igemm_fwd: producer warpgroup + two consumer warpgroups
 constexpr int kMaxTaps = 64;
 
+// Registers per thread after the k_igemm_fwd warpgroups re-balance them: the launch gives 168 to each of the 384 threads
+// (65536 / 384, rounded down to a multiple of 8), and an increase waits until the producer's decrease has freed enough,
+// so the two must add up to no more than the launch allocation.  The producer gets 56, not the usual 40: its K walk keeps
+// the KSkip state, the im2col coordinates and (MULTI) the class decode live, and ptxas spills it to local memory at 40
+// (every instantiation) and at 48 (both MULTI instantiations).  224 is what is left for the consumers, enough for the 128
+// accumulators of BLOCK_N = 128 plus the epilogue without spills.
+constexpr int kFwdProducerRegs = 56, kFwdConsumerRegs = 224;
+static_assert(kFwdProducerRegs * 128 + kFwdConsumerRegs * 256 <= 168 * kFwdThreads, "fwd register split");
+
 // smem pipeline depth of the fwd kernel: stage = A tile (16 KB) + weight tile (8 or 16 KB)
-__host__ __device__ constexpr int fwd_stages(int block_n) { return block_n == 128 ? 4 : 6; }
-// fwd smem besides the stages: fp32 accumulator exchange tile (128 x BLOCK_N), 8 x 4 KB epilogue staging, alignment
-// slack and barriers
-__host__ __device__ constexpr int fwd_tail(int block_n) { return kBlockM * block_n * 4 + 8 * 32 * 128 + 1024 + 512; }
+__host__ __device__ constexpr int fwd_stages(int block_n) { return block_n == 128 ? 5 : 8; }
+// epilogue staging tile of one consumer warpgroup: 128 rows x BLOCK_N bf16, as 64-column sub-tiles of 16 KB
+__host__ __device__ constexpr int fwd_stg_bytes(int block_n) { return kBlockM * block_n * 2; }
+// fwd smem: the stages, both consumers' staging tiles, alignment slack and barriers
+__host__ __device__ constexpr int fwd_smem(int block_n) {
+  return fwd_stages(block_n) * (kBlockM * kBlockK * 2 + block_n * kBlockK * 2) + 2 * fwd_stg_bytes(block_n) + 1024 + 512;
+}
 
 struct TapEntry { uint16_t off_w, off_h; int32_t kofs; };
 
@@ -180,16 +199,23 @@ __device__ __forceinline__ void decode_tile(const FwdParams& p, int tile, int n_
   m_g = local / n_tiles; n_t = local - m_g * n_tiles;     // m-major: CTAs running together share A tiles, weights stay in L2
 }
 
-// One warpgroup's share of a K block of the fwd GEMM: D[64 x BLOCK_N] (+)= A[64 x 64] * B[BLOCK_N x 64]^T, both K-major.
+// A K block of the fwd GEMM for one consumer warpgroup: D[128 x BLOCK_N] (+)= A[128 x 64] * B[BLOCK_N x 64]^T, both
+// K-major; rows 0..63 accumulate into acc[0 .. BLOCK_N/2), rows 64..127 into acc[BLOCK_N/2 .. BLOCK_N).
 template <int BLOCK_N>
-__device__ __forceinline__ void fwd_mma_block(float (&acc)[BLOCK_N / 2], uint32_t a_addr, uint32_t b_addr, uint32_t accumulate) {
+__device__ __forceinline__ void fwd_mma_block(float (&acc)[BLOCK_N], uint32_t a_addr, uint32_t b_addr, uint32_t accumulate) {
   const uint64_t adesc = make_smem_desc(a_addr, 16, 1024);
+  const uint64_t adesc_hi = make_smem_desc(a_addr + 64 * kBlockK * 2, 16, 1024);
   const uint64_t bdesc = make_smem_desc(b_addr, 16, 1024);
 #pragma unroll
   for (int k = 0; k < kBlockK / 16; ++k) {
     // advance 16 elements (32 B) along K inside the 128-B swizzle row: +2 in 16-B units
-    if constexpr (BLOCK_N == 128) wgmma_m64n128<0, 0>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), accumulate | (uint32_t)k);
-    else wgmma_m64n64<0, 0>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), accumulate | (uint32_t)k);
+    if constexpr (BLOCK_N == 128) {
+      wgmma_m64n128<0, 0>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), accumulate | (uint32_t)k);
+      wgmma_m64n128<0, 0>(acc + BLOCK_N / 2, adesc_hi + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), accumulate | (uint32_t)k);
+    } else {
+      wgmma_m64n64<0, 0>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), accumulate | (uint32_t)k);
+      wgmma_m64n64<0, 0>(acc + BLOCK_N / 2, adesc_hi + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), accumulate | (uint32_t)k);
+    }
   }
 }
 
@@ -202,11 +228,19 @@ __device__ __forceinline__ void fwd_mma_block(float (&acc)[BLOCK_N / 2], uint32_
 // matching y values, applies the ReLU gate, stores g and adds sum(g), sum(g * xhat) of its 8 channels x 8 rows; rows are
 // then combined by the same fixed-order xor tree as the forward statistics.  Output: g, and [32-row group][2][N] partials.
 //
-// The accumulators leave the registers through an fp32 exchange tile in shared memory (16-byte chunk j of row r is
-// stored at chunk j ^ (r & 7): conflict-free for both the fragment stores and the row reads), so that each epilogue lane
-// owns one output row, as the coalesced staged stores and the 32-row statistics groups need.
+// Ping-pong: the CTA's w-th work item belongs to consumer warpgroup w & 1.  The two mainloops take turns through a pair
+// of mbarriers (order_bar): a consumer starts its K loop once the other one has issued the last MMA of the previous
+// item, so the MMAs of one tile run while the other warpgroup drains its epilogue.  With the turn it hands over the
+// position in the stage ring (stage, phase) where its K loop ended, so neither consumer has to count the K blocks of
+// the other's items (dense walk, K-block skipping and classes without taps all hand over the same way).  Taking turns
+// is also what keeps the ring consistent: a consumer only waits on stages whose earlier fills have all been consumed.
+//
+// Epilogue, per 64-column chunk: every thread converts its own accumulator fragments (+ bias, + addend, round to bf16)
+// and writes them into the warpgroup's 128 x 64 bf16 staging tile (16-byte chunk j of row r at chunk j ^ (r & 7):
+// conflict-free for the fragment stores and for the row reads); after a warpgroup barrier, warp q reads rows
+// 32q .. 32q+31 back row-coalesced for full-line stores, the BatchNorm statistics and the BNB gate.
 template <int BLOCK_N, bool MULTI, bool BNB>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kFwdThreads, 1)
 k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ FwdParams p) {
   static_assert(BLOCK_N == 64 || BLOCK_N == 128, "wgmma N of the fwd kernel");
@@ -218,11 +252,13 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   pdl_trigger();
-  constexpr int kStgBytes = 32 * 128;                      // one epilogue warp's 32 rows x 64 bf16 columns
-  float* const acc_tile = (float*)(smem + kStages * kStageBytes);     // 128 x BLOCK_N fp32
-  uint8_t* stg_base = (uint8_t*)(acc_tile + kBlockM * BLOCK_N);       // 8 warps x 4 KB (1024-B aligned)
-  uint64_t* full_bar = (uint64_t*)(stg_base + 8 * kStgBytes);
+  constexpr int kStgBytes = fwd_stg_bytes(BLOCK_N);
+  constexpr int kChunkStg = kBlockM * 64 * 2;                         // one 64-column sub-tile of the staging tile
+  uint8_t* const stg_base = smem + kStages * kStageBytes;             // one staging tile per consumer (1024-B aligned)
+  uint64_t* full_bar = (uint64_t*)(stg_base + 2 * kStgBytes);
   uint64_t* empty_bar = full_bar + kStages;
+  uint64_t* order_bar = empty_bar + kStages;                          // [consumer]: its turn to run a mainloop
+  int* ring_pos = (int*)(order_bar + 2);                              // stage * 2 + phase handed over with the turn
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_tiles = (p.N + BLOCK_N - 1) / BLOCK_N;
@@ -240,16 +276,18 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
   if (threadIdx.x == 0) {
     for (int j = 0; j < p.ncls; ++j) prefetch_tmap(&tmA.m[j]);
     prefetch_tmap(&tmB);
-    // empty: one arrival per consumer warpgroup once its MMAs have read the stage
-    for (int i = 0; i < kStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kConsumers / 128); }
+    // empty: one arrival by the consumer warpgroup whose MMAs have read the stage
+    for (int i = 0; i < kStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
+    mbar_init(&order_bar[0], 1); mbar_init(&order_bar[1], 1);
     fence_mbar_init();
   }
   __syncthreads();
   pdl_wait();          // barrier set-up and descriptor prefetch above overlap the previous grid's tail; global memory from here on
 
-  if (warp == kProducerWarp) {
+  if (warp < 4) {
     // ------------------------------ TMA producer ------------------------------
-    if (lane == 0) {
+    setmaxnreg_dec<kFwdProducerRegs>();
+    if (threadIdx.x == 0) {
       int stage = 0; uint32_t phase = 0;
       const uint32_t* const km = live_kmask(p.kmask, p.kmask_words, p.N);
       for (int w = 0; w < my_items; ++w) {
@@ -296,41 +334,82 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
       }
     }
   } else {
-    // ------------------------------ consumers: MMA, then epilogue ------------------------------
-    const int wg = warp >> 2;                 // MMA: rows 64*wg .. 64*wg+63 of the tile
-    const int quarter = warp & 3;             // epilogue: rows 32*quarter .. +31 of the tile, one per lane
-    const int half = warp >> 2;               // epilogue: which half of the 64-column chunks this warp drains
-    const int erow = quarter * 32 + lane;
-    int stage = 0; uint32_t phase = 0;
+    // ------------------------------ consumers: MMA and epilogue of every other work item ------------------------------
+    setmaxnreg_inc<kFwdConsumerRegs>();
+    const int cw = (warp >> 2) - 1;           // consumer warpgroup: work items cw, cw + 2, cw + 4, ...
+    const int q = warp & 3;                   // epilogue: rows 32q .. 32q+31 of the tile, one per lane
+    const int wtid = threadIdx.x & 127;
+    const int bar_id = 1 + cw;                // warpgroup-local named barrier
     const uint32_t* const km = live_kmask(p.kmask, p.kmask_words, p.N);
-    // 32 fp32 accumulators of this lane's row, columns c .. c+31, from the exchange tile
-    auto acc_row_ld = [&](int c, uint32_t* v) {
-      const uint32_t rb = smem_u32(acc_tile) + (uint32_t)(erow * BLOCK_N * 4);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const uint4 t = lds128(rb + ((uint32_t)(((c >> 2) + i) ^ (erow & 7)) << 4));
-        v[4 * i] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
-      }
-    };
-    for (int w = 0; w < my_items; ++w) {
+    const uint32_t stg = smem_u32(stg_base + cw * kStgBytes);
+    // fragment rows of this thread: fr0 + 8h + 64mh (h, mh in {0, 1}); their swizzle key (row & 7) is lane / 4
+    const int fr0 = q * 16 + (lane >> 2);
+    const uint32_t fsw = (uint32_t)(lane >> 2);
+    const uint32_t frag_base = stg + (uint32_t)(fr0 * 128 + (lane & 3) * 4);
+    // row-read geometry of this lane: rows r_in + 4i of the warp's 32, 16-byte column c16 of each 128-byte row
+    const int r_in = lane >> 3, c16 = lane & 7;
+    const uint32_t buf = stg + (uint32_t)(q * 32 * 128);
+    const uint32_t rd_even = buf + r_in * 128 + ((uint32_t)(c16 ^ r_in) << 4);          // rows r_in + 8j
+    const uint32_t rd_odd = buf + (r_in + 4) * 128 + ((uint32_t)(c16 ^ (r_in + 4)) << 4);  // rows r_in + 4 + 8j
+    for (int it = 0, w = cw; w < my_items; ++it, w += 2) {
       int ci, m_g, n_t; get_tile(w, ci, m_g, n_t);
       const ClsEntry& ce = p.cls[MULTI ? ci : 0];
       const bool has_acc = MULTI ? ce.ntaps > 0 : true;   // a class no tap reaches: the accumulator was never written, its value is zero
       const int m_t = m_g;
-      const int row = m_t * kBlockM + quarter * 32 + lane;
-      const bool row_ok = row < ce.M;
-      long long opix = 0;
-      if (row_ok && !p.staged_store) {    // generic output mapping, one division chain per tile
-        opix = row;
-        if (MULTI || !p.linear) {
-          int n, pp, qq; decompose_pixel(row, ce.P_it, ce.Q_it, n, pp, qq);
-          opix = (long long)n * p.out_img_pix + (long long)(pp * p.osh + ce.oah) * p.out_row_pix + (qq * p.osw + ce.oaw);
-        }
+
+      // ---- mainloop, in turn with the other consumer ----
+      int stage = 0; uint32_t phase = 0;
+      const int turn = it + cw;               // turns of this consumer before this item (item 0 needs none)
+      if (turn > 0) {
+        mbar_wait(&order_bar[cw], (uint32_t)((turn - 1) & 1));
+        const int pos = *(volatile int*)ring_pos;
+        stage = pos >> 1; phase = (uint32_t)(pos & 1);
       }
-      __nv_bfloat16* orow = p.out + opix * p.ldc;
-      // staged-path geometry of this lane: rows r_in + 4i of the warp's 32, 16-byte column c16 of each 128-byte row
-      const int r_in = lane >> 3, c16 = lane & 7;
-      const long long wrow0 = (long long)m_t * kBlockM + quarter * 32;        // first row of this warp's 32
+      // every warp of the warpgroup has taken its turn and read the ring position before one thread passes the turn on
+      // (which rewrites the position and may let the other consumer complete the next phase of order_bar[cw]); the
+      // MMAs do not order this: an item of one K block passes the turn before its MMA is known to be issued by all warps
+      bar_sync(bar_id, 128);
+      auto pass_turn = [&]() {
+        if (wtid == 0) { *(volatile int*)ring_pos = stage * 2 + (int)phase; mbar_arrive(&order_bar[cw ^ 1]); }
+      };
+      float acc[BLOCK_N];
+      if (has_acc) {
+#pragma unroll
+        for (int i = 0; i < BLOCK_N; ++i) acc[i] = 0.f;
+        int prev = -1;                        // stage of the previous K block: freed once its MMAs have completed
+        auto mma_block = [&](uint32_t accumulate) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint32_t s_addr = smem_u32(smem + stage * kStageBytes);
+          wgmma_fence();
+          fwd_mma_block<BLOCK_N>(acc, s_addr, s_addr + kABytes, accumulate);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (prev >= 0 && wtid == 0) mbar_arrive(&empty_bar[prev]);
+          prev = stage;
+          if (++stage == kStages) { stage = 0; phase ^= 1; }
+        };
+        // one walk with a single MMA call site (two would make ptxas serialise the wgmma pipeline)
+        KSkip ks; uint32_t any = 0;
+        if (km) ks.begin(km, p.kmask_words, n_t * BLOCK_N, BLOCK_N, p.N);
+        for (int tap = 0; tap < ce.ntaps; ++tap) {
+          const int kb0 = p.taps[(MULTI ? ce.tap0 : 0) + tap].kofs >> 6;
+          for (int cc = 0; cc < p.cchunks; ++cc) {
+            const bool last = tap == ce.ntaps - 1 && cc == p.cchunks - 1;
+            if (km && !ks.take(kb0 + cc, last, any)) continue;
+            mma_block(any);
+            any = 1;
+          }
+        }
+        pass_turn();                          // every MMA of this tile is issued: the other consumer's K loop may start
+        wgmma_wait<0>();
+        acc_fence(acc);
+        if (prev >= 0 && wtid == 0) mbar_arrive(&empty_bar[prev]);
+      } else {
+        pass_turn();
+      }
+
+      // ---- epilogue ----
+      const long long wrow0 = (long long)m_t * kBlockM + q * 32;        // first row of this warp's 32
       const int rows_left = (int)(ce.M - wrow0 < 32 ? (ce.M - wrow0 < 0 ? 0 : ce.M - wrow0) : 32);
       const long long ldc = p.ldc;
       const int N = p.N;
@@ -351,10 +430,10 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
       auto row_off = [&](int i) -> long long { return MULTI ? ooff[MULTI ? i : 0] : rbase + (long long)(i * 4) * ldc; };
       if (MULTI && !has_acc) {
         // parity class no tap reaches (e.g. 3 of the 4 classes of a 1x1 stride-2 convolution): dX there is the fused addend
-        // or zero — plain coalesced copies / stores; no accumulator exists, so no hand-shake with the MMA thread either
+        // or zero — plain coalesced copies / stores
         if (p.staged_store) {
 #pragma unroll 1
-          for (int c = half * 64; c < BLOCK_N; c += 128) {
+          for (int c = 0; c < BLOCK_N; c += 64) {
             const int n0 = n_t * BLOCK_N + c;
             if (n0 >= N) break;
             if (n0 + c16 * 8 + 8 > N) continue;
@@ -368,144 +447,92 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
             for (int i = 0; i < 8; ++i)
               if (i * 4 + r_in < rows_left) *reinterpret_cast<uint4*>(p.out + row_off(i) + n0) = z[i];
           }
-        } else if (row_ok && half == 0) {
-          for (int j = n_t * BLOCK_N; j < min(p.N, (n_t + 1) * BLOCK_N); ++j)
-            orow[j] = p.addend ? p.addend[opix * p.ldc + j] : __float2bfloat16_rn(0.f);
+        } else {
+          const int row = m_t * kBlockM + wtid;
+          if (row < ce.M) {
+            int n, pp, qq; decompose_pixel(row, ce.P_it, ce.Q_it, n, pp, qq);
+            const long long opix = (long long)n * p.out_img_pix + (long long)(pp * p.osh + ce.oah) * p.out_row_pix + (qq * p.osw + ce.oaw);
+            for (int j = n_t * BLOCK_N; j < min(p.N, (n_t + 1) * BLOCK_N); ++j)
+              p.out[opix * p.ldc + j] = p.addend ? p.addend[opix * p.ldc + j] : __float2bfloat16_rn(0.f);
+          }
         }
         continue;
       }
-      {
-        // ---- mainloop: this warpgroup's 64 x BLOCK_N accumulators over the tile's K blocks ----
-        float acc[BLOCK_N / 2];
-#pragma unroll
-        for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
-        int prev = -1;                        // stage of the previous K block: freed once its MMAs have completed
-        auto mma_block = [&](uint32_t accumulate) {
-          mbar_wait(&full_bar[stage], phase);
-          const uint32_t s_addr = smem_u32(smem + stage * kStageBytes);
-          wgmma_fence();
-          fwd_mma_block<BLOCK_N>(acc, s_addr + (uint32_t)(wg * (kABytes / 2)), s_addr + kABytes, accumulate);
-          wgmma_commit();
-          wgmma_wait<1>();
-          if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
-          prev = stage;
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        };
-        // one walk with a single MMA call site (two would make ptxas serialise the wgmma pipeline)
-        KSkip ks; uint32_t any = 0;
-        if (km) ks.begin(km, p.kmask_words, n_t * BLOCK_N, BLOCK_N, p.N);
-        for (int tap = 0; tap < ce.ntaps; ++tap) {
-          const int kb0 = p.taps[(MULTI ? ce.tap0 : 0) + tap].kofs >> 6;
-          for (int cc = 0; cc < p.cchunks; ++cc) {
-            const bool last = tap == ce.ntaps - 1 && cc == p.cchunks - 1;
-            if (km && !ks.take(kb0 + cc, last, any)) continue;
-            mma_block(any);
-            any = 1;
-          }
-        }
-        wgmma_wait<0>();
-        acc_fence(acc);
-        if (prev >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev]);
-        // ---- registers -> exchange tile (once the previous tile's epilogue has finished reading it) ----
-        bar_sync(1, kConsumers);
-        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-#pragma unroll
-        for (int j = 0; j < BLOCK_N / 8; ++j)
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int r = r0 + 8 * h, col = 8 * j + 2 * (lane & 3);
-            *reinterpret_cast<float2*>(acc_tile + r * BLOCK_N + (((col >> 2) ^ (r & 7)) << 2) + (col & 3)) =
-                make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-          }
-        bar_sync(1, kConsumers);
-      }
       if (p.staged_store) {
-        // accumulators -> registers -> 128B-swizzled smem sub-tile (32 rows x 64 cols) -> coalesced global
-        // stores, so every output line leaves the SM as full 128-byte rows instead of 32 scattered 16-byte pieces.
-        // Everything that does not depend on the column chunk is hoisted (row pointers, validity, swizzled
-        // staging offsets) and the staging buffer is addressed through the shared window (st/ld.shared, not
-        // generic loads and stores, which are slower on shared memory).
-        const uint32_t buf = smem_u32(stg_base + warp * kStgBytes);
+        // fragments -> bf16 staging tile -> coalesced global stores, so every output line leaves the SM as full 128-byte
+        // rows instead of scattered 4-byte pieces.  The staging tile is addressed through the shared window (st/ld.shared,
+        // not generic loads and stores, which are slower on shared memory).
         __nv_bfloat16* const gout = p.out;
         const __nv_bfloat16* const gadd = p.addend;
         const float* bias = p.bias;
-        float* stats = p.stats ? p.stats + (long long)(m_t * 4 + quarter) * 2 * N + c16 * 8 : nullptr;
-        const uint32_t wr_base = buf + lane * 128;                              // my row in the staging tile
-        const uint32_t wr_sw = (uint32_t)(lane & 7);
-        const uint32_t rd_even = buf + r_in * 128 + ((uint32_t)(c16 ^ r_in) << 4);          // rows r_in + 8j
-        const uint32_t rd_odd = buf + (r_in + 4) * 128 + ((uint32_t)(c16 ^ (r_in + 4)) << 4);  // rows r_in + 4 + 8j
-        uint4 a_pref[8];
+        float* stats = p.stats ? p.stats + (long long)(m_t * 4 + q) * 2 * N + c16 * 8 : nullptr;
+        if (gadd) {
+          // addend tile, coalesced (8 lanes cover one 128-byte row, 4 rows per instruction), staged into the warp's own
+          // 32 rows; the fragment pass below reads it back at its fragment positions
+          __syncwarp();                       // the warp's row reads of the previous tile are done
+#pragma unroll
+          for (int ch = 0; ch < BLOCK_N / 64; ++ch) {
+            const int n0 = n_t * BLOCK_N + ch * 64;
+            if (n0 >= N) break;
+            const bool col_ok = n0 + c16 * 8 + 8 <= N;
+            uint4 a[8];
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              a[i] = make_uint4(0u, 0u, 0u, 0u);
+              if (i * 4 + r_in < rows_left && col_ok) a[i] = *reinterpret_cast<const uint4*>(gadd + row_off(i) + n0);
+            }
+#pragma unroll
+            for (int i = 0; i < 8; ++i) sts128(((i & 1) ? rd_odd : rd_even) + (uint32_t)(ch * kChunkStg + (i >> 1) * 1024), a[i]);
+          }
+        }
+        // the staging tile is free (every warp has read the previous tile back) and the staged addend is visible
+        bar_sync(bar_id, 128);
+#pragma unroll
+        for (int ch = 0; ch < BLOCK_N / 64; ++ch) {
+          const int n0 = n_t * BLOCK_N + ch * 64;
+          if (n0 >= N) break;
+#pragma unroll
+          for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+              for (int j = 0; j < 8; ++j) {
+                const int i = mh * (BLOCK_N / 2) + 4 * (ch * 8 + j) + 2 * h;
+                float f0 = acc[i], f1 = acc[i + 1];
+                const int n = n0 + 8 * j + 2 * (lane & 3);
+                if (bias) {
+                  if (n < N) f0 += bias[n];
+                  if (n + 1 < N) f1 += bias[n + 1];
+                }
+                const uint32_t addr = frag_base + (uint32_t)(ch * kChunkStg + (64 * mh + 8 * h) * 128) + (((uint32_t)j ^ fsw) << 4);
+                if (gadd) {       // fused skip-gradient accumulation, in fp32 before the one rounding to bf16
+                  const uint32_t a = lds32(addr);
+                  const float2 t2 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&a));
+                  f0 += t2.x; f1 += t2.y;
+                }
+                const __nv_bfloat162 hv = __floats2bfloat162_rn(f0, f1);
+                sts32(addr, *reinterpret_cast<const uint32_t*>(&hv));
+              }
+        }
+        bar_sync(bar_id, 128);
 #pragma unroll 1
-        for (int c = half * 64; c < BLOCK_N; c += 128) {
-          const int n0 = n_t * BLOCK_N + c;
+        for (int ch = 0; ch < BLOCK_N / 64; ++ch) {
+          const int n0 = n_t * BLOCK_N + ch * 64;
           if (n0 >= N) break;
           const bool col_ok = n0 + c16 * 8 + 8 <= N;
-          // both 32-column halves of the chunk are requested before the one wait
-          uint32_t v[64];
-          acc_row_ld(c, v);
-          acc_row_ld(c + 32, v + 32);
-          if (gadd) {
-            // addend sub-tile of THIS chunk was prefetched into registers one chunk earlier (coalesced: 8 lanes
-            // cover one 128-byte row, 4 rows per instruction); stage it, then prefetch the next chunk's
-            if (c == half * 64) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                a_pref[i] = make_uint4(0u, 0u, 0u, 0u);
-                if (i * 4 + r_in < rows_left && col_ok) a_pref[i] = *reinterpret_cast<const uint4*>(gadd + row_off(i) + n0);
-              }
-            }
-#pragma unroll
-            for (int i = 0; i < 8; ++i) sts128(((i & 1) ? rd_odd : rd_even) + (uint32_t)((i >> 1) * 1024), a_pref[i]);
-            if (c + 128 < BLOCK_N && n0 + 128 < N) {
-              const bool col_ok2 = n0 + 128 + c16 * 8 + 8 <= N;
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                a_pref[i] = make_uint4(0u, 0u, 0u, 0u);
-                if (i * 4 + r_in < rows_left && col_ok2) a_pref[i] = *reinterpret_cast<const uint4*>(gadd + row_off(i) + n0 + 128);
-              }
-            }
-            __syncwarp();
-          }
-#pragma unroll
-          for (int j = 0; j < 64; j += 8) {
-            float f[8];
-#pragma unroll
-            for (int q = 0; q < 8; ++q) f[q] = __uint_as_float(v[j + q]);
-            if (bias) {
-#pragma unroll
-              for (int q = 0; q < 8; ++q) if (n0 + j + q < N) f[q] += bias[n0 + j + q];
-            }
-            const uint32_t waddr = wr_base + (((uint32_t)(j >> 3) ^ wr_sw) << 4);   // 16-byte chunk j/8 of my row, swizzled
-            if (gadd) {
-              // fused skip-gradient accumulation: each thread reads its own row of the staged addend back before
-              // overwriting it with the result
-              const uint4 a = lds128(waddr);
-              const __nv_bfloat162* ah = reinterpret_cast<const __nv_bfloat162*>(&a);
-#pragma unroll
-              for (int q = 0; q < 4; ++q) { const float2 t2 = __bfloat1622float2(ah[q]); f[2 * q] += t2.x; f[2 * q + 1] += t2.y; }
-            }
-            __nv_bfloat162 h0 = __floats2bfloat162_rn(f[0], f[1]);
-            __nv_bfloat162 h1 = __floats2bfloat162_rn(f[2], f[3]);
-            __nv_bfloat162 h2 = __floats2bfloat162_rn(f[4], f[5]);
-            __nv_bfloat162 h3 = __floats2bfloat162_rn(f[6], f[7]);
-            uint4 pk;
-            pk.x = *(uint32_t*)&h0; pk.y = *(uint32_t*)&h1; pk.z = *(uint32_t*)&h2; pk.w = *(uint32_t*)&h3;
-            sts128(waddr, pk);
-          }
-          __syncwarp();
           // smem -> global, coalesced: 8 lanes write one full 128-byte output row, 4 rows per instruction.
-          // Plain stores are fire-and-forget, so the staging buffer is free again after this read-back
-          // (a TMA store here would make every chunk wait for the previous store to drain).
+          // Plain stores are fire-and-forget, so the staging tile is free again after this read-back
+          // (a TMA store here would make every tile wait for the previous store to drain).
           uint4 o[8];
 #pragma unroll
-          for (int i = 0; i < 8; ++i) o[i] = lds128(((i & 1) ? rd_odd : rd_even) + (uint32_t)((i >> 1) * 1024));
+          for (int i = 0; i < 8; ++i) o[i] = lds128(((i & 1) ? rd_odd : rd_even) + (uint32_t)(ch * kChunkStg + (i >> 1) * 1024));
           // per-channel sums of the row-coalesced view: this lane owns channels n0 + c16*8 .. +8 of rows r_in + 4i.
           // BNB: sum g and sum g * xhat of the gradient, gated before it is stored; otherwise (stats) the BatchNorm batch statistics sum o and
           // sum o^2 of exactly the values stored (bf16-rounded).  A fixed-order xor tree over the 4 row groups finishes
           // the 32 rows.
           float s1[8], s2[8];
 #pragma unroll
-          for (int q = 0; q < 8; ++q) { s1[q] = 0.f; s2[q] = 0.f; }
+          for (int qq = 0; qq < 8; ++qq) { s1[qq] = 0.f; s2[qq] = 0.f; }
           if (BNB) {
             uint4 yv[8];
 #pragma unroll
@@ -517,21 +544,21 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
             if (col_ok) {
               const int cb = n0 + c16 * 8;
 #pragma unroll
-              for (int q = 0; q < 8; q += 4) {
+              for (int qq = 0; qq < 8; qq += 4) {
                 const float4 one4 = make_float4(1.f, 1.f, 1.f, 1.f), zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
-                const float4 a4 = p.bn_weight ? *reinterpret_cast<const float4*>(p.bn_weight + cb + q) : one4;
-                const float4 b4 = p.bn_bias ? *reinterpret_cast<const float4*>(p.bn_bias + cb + q) : zero4;
-                const float4 m4 = *reinterpret_cast<const float4*>(p.bn_mean + cb + q), i4 = *reinterpret_cast<const float4*>(p.bn_invstd + cb + q);
-                is_[q] = i4.x; is_[q + 1] = i4.y; is_[q + 2] = i4.z; is_[q + 3] = i4.w;
-                nm[q] = m4.x; nm[q + 1] = m4.y; nm[q + 2] = m4.z; nm[q + 3] = m4.w;
+                const float4 a4 = p.bn_weight ? *reinterpret_cast<const float4*>(p.bn_weight + cb + qq) : one4;
+                const float4 b4 = p.bn_bias ? *reinterpret_cast<const float4*>(p.bn_bias + cb + qq) : zero4;
+                const float4 m4 = *reinterpret_cast<const float4*>(p.bn_mean + cb + qq), i4 = *reinterpret_cast<const float4*>(p.bn_invstd + cb + qq);
+                is_[qq] = i4.x; is_[qq + 1] = i4.y; is_[qq + 2] = i4.z; is_[qq + 3] = i4.w;
+                nm[qq] = m4.x; nm[qq + 1] = m4.y; nm[qq + 2] = m4.z; nm[qq + 3] = m4.w;
                 // scale / shift exactly as k_bn_finalize_stats computed them for the forward apply pass
-                sc[q] = a4.x * i4.x; sc[q + 1] = a4.y * i4.y; sc[q + 2] = a4.z * i4.z; sc[q + 3] = a4.w * i4.w;
-                sf[q] = fmaf(-m4.x, sc[q], b4.x); sf[q + 1] = fmaf(-m4.y, sc[q + 1], b4.y);
-                sf[q + 2] = fmaf(-m4.z, sc[q + 2], b4.z); sf[q + 3] = fmaf(-m4.w, sc[q + 3], b4.w);
+                sc[qq] = a4.x * i4.x; sc[qq + 1] = a4.y * i4.y; sc[qq + 2] = a4.z * i4.z; sc[qq + 3] = a4.w * i4.w;
+                sf[qq] = fmaf(-m4.x, sc[qq], b4.x); sf[qq + 1] = fmaf(-m4.y, sc[qq + 1], b4.y);
+                sf[qq + 2] = fmaf(-m4.z, sc[qq + 2], b4.z); sf[qq + 3] = fmaf(-m4.w, sc[qq + 3], b4.w);
               }
             } else {
 #pragma unroll
-              for (int q = 0; q < 8; ++q) { sc[q] = 0.f; sf[q] = 0.f; is_[q] = 0.f; nm[q] = 0.f; }
+              for (int qq = 0; qq < 8; ++qq) { sc[qq] = 0.f; sf[qq] = 0.f; is_[qq] = 0.f; nm[qq] = 0.f; }
             }
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
@@ -539,15 +566,15 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
                 __nv_bfloat162* gh = reinterpret_cast<__nv_bfloat162*>(&o[i]);
                 const __nv_bfloat162* yh = reinterpret_cast<const __nv_bfloat162*>(&yv[i]);
 #pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  float2 d2 = __bfloat1622float2(gh[q]);
-                  const float2 y2 = __bfloat1622float2(yh[q]);
+                for (int qq = 0; qq < 4; ++qq) {
+                  float2 d2 = __bfloat1622float2(gh[qq]);
+                  const float2 y2 = __bfloat1622float2(yh[qq]);
                   // the forward wrote z = max(fma(y, scale, shift), 0): same expression, same operands -> same decision
-                  if (!(fmaf(y2.x, sc[2 * q], sf[2 * q]) > 0.f)) d2.x = 0.f;
-                  if (!(fmaf(y2.y, sc[2 * q + 1], sf[2 * q + 1]) > 0.f)) d2.y = 0.f;
-                  gh[q] = __floats2bfloat162_rn(d2.x, d2.y);                    // exact: d2 is a bf16 value or zero
-                  s1[2 * q] += d2.x;     s2[2 * q] = fmaf(d2.x, (y2.x - nm[2 * q]) * is_[2 * q], s2[2 * q]);
-                  s1[2 * q + 1] += d2.y; s2[2 * q + 1] = fmaf(d2.y, (y2.y - nm[2 * q + 1]) * is_[2 * q + 1], s2[2 * q + 1]);
+                  if (!(fmaf(y2.x, sc[2 * qq], sf[2 * qq]) > 0.f)) d2.x = 0.f;
+                  if (!(fmaf(y2.y, sc[2 * qq + 1], sf[2 * qq + 1]) > 0.f)) d2.y = 0.f;
+                  gh[qq] = __floats2bfloat162_rn(d2.x, d2.y);                    // exact: d2 is a bf16 value or zero
+                  s1[2 * qq] += d2.x;     s2[2 * qq] = fmaf(d2.x, (y2.x - nm[2 * qq]) * is_[2 * qq], s2[2 * qq]);
+                  s1[2 * qq + 1] += d2.y; s2[2 * qq + 1] = fmaf(d2.y, (y2.y - nm[2 * qq + 1]) * is_[2 * qq + 1], s2[2 * qq + 1]);
                 }
               }
             }
@@ -561,19 +588,19 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
               if (i * 4 + r_in < rows_left) {
                 const __nv_bfloat162* h2 = reinterpret_cast<const __nv_bfloat162*>(&o[i]);
 #pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const float2 t2 = __bfloat1622float2(h2[q]);
-                  s1[2 * q] += t2.x; s2[2 * q] = fmaf(t2.x, t2.x, s2[2 * q]);
-                  s1[2 * q + 1] += t2.y; s2[2 * q + 1] = fmaf(t2.y, t2.y, s2[2 * q + 1]);
+                for (int qq = 0; qq < 4; ++qq) {
+                  const float2 t2 = __bfloat1622float2(h2[qq]);
+                  s1[2 * qq] += t2.x; s2[2 * qq] = fmaf(t2.x, t2.x, s2[2 * qq]);
+                  s1[2 * qq + 1] += t2.y; s2[2 * qq + 1] = fmaf(t2.y, t2.y, s2[2 * qq + 1]);
                 }
               }
             }
           }
           if (BNB || stats) {
 #pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              s1[q] += __shfl_xor_sync(0xffffffffu, s1[q], 8);  s2[q] += __shfl_xor_sync(0xffffffffu, s2[q], 8);
-              s1[q] += __shfl_xor_sync(0xffffffffu, s1[q], 16); s2[q] += __shfl_xor_sync(0xffffffffu, s2[q], 16);
+            for (int qq = 0; qq < 8; ++qq) {
+              s1[qq] += __shfl_xor_sync(0xffffffffu, s1[qq], 8);  s2[qq] += __shfl_xor_sync(0xffffffffu, s2[qq], 8);
+              s1[qq] += __shfl_xor_sync(0xffffffffu, s1[qq], 16); s2[qq] += __shfl_xor_sync(0xffffffffu, s2[qq], 16);
             }
             if (r_in == 0 && col_ok) {
               float4* d1 = reinterpret_cast<float4*>(stats + n0);
@@ -582,43 +609,33 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
               d2[0] = make_float4(s2[0], s2[1], s2[2], s2[3]); d2[1] = make_float4(s2[4], s2[5], s2[6], s2[7]);
             }
           }
-          __syncwarp();
         }
       } else {
-#pragma unroll 1
-      for (int c = half * 32; c < BLOCK_N; c += 64) {
-        uint32_t v[32];
-        acc_row_ld(c, v);
-        const int n0 = n_t * BLOCK_N + c;
-        if (row_ok && n0 < p.N) {
-          float f[32];
+        // generic output mapping: every thread stores its own fragments (4 rows, 2 adjacent columns per 8)
 #pragma unroll
-          for (int j = 0; j < 32; ++j) f[j] = __uint_as_float(v[j]);
-          if (p.bias) {
+        for (int mh = 0; mh < 2; ++mh)
 #pragma unroll
-            for (int j = 0; j < 32; ++j) if (n0 + j < p.N) f[j] += p.bias[n0 + j];
-          }
-          if (p.addend) {
-            const __nv_bfloat16* ar = p.addend + opix * p.ldc + n0;
-            for (int j = 0; j < 32; ++j) if (n0 + j < p.N) f[j] += __bfloat162float(ar[j]);
-          }
-          __nv_bfloat16* dst = orow + n0;
-          if (n0 + 32 <= p.N && (((uintptr_t)dst) & 15) == 0) {
-#pragma unroll
-            for (int j = 0; j < 32; j += 8) {
-              __nv_bfloat162 h0 = __floats2bfloat162_rn(f[j], f[j + 1]);
-              __nv_bfloat162 h1 = __floats2bfloat162_rn(f[j + 2], f[j + 3]);
-              __nv_bfloat162 h2 = __floats2bfloat162_rn(f[j + 4], f[j + 5]);
-              __nv_bfloat162 h3 = __floats2bfloat162_rn(f[j + 6], f[j + 7]);
-              uint4 pk;
-              pk.x = *(uint32_t*)&h0; pk.y = *(uint32_t*)&h1; pk.z = *(uint32_t*)&h2; pk.w = *(uint32_t*)&h3;
-              *(uint4*)(dst + j) = pk;
+          for (int h = 0; h < 2; ++h) {
+            const int row = m_t * kBlockM + fr0 + 8 * h + 64 * mh;
+            if (row >= ce.M) continue;
+            long long opix = row;
+            if (MULTI || !p.linear) {
+              int n, pp, qq; decompose_pixel(row, ce.P_it, ce.Q_it, n, pp, qq);
+              opix = (long long)n * p.out_img_pix + (long long)(pp * p.osh + ce.oah) * p.out_row_pix + (qq * p.osw + ce.oaw);
             }
-          } else {
-            for (int j = 0; j < 32; ++j) if (n0 + j < p.N) dst[j] = __float2bfloat16_rn(f[j]);
+            __nv_bfloat16* const orow = p.out + opix * p.ldc;
+#pragma unroll
+            for (int j = 0; j < BLOCK_N / 8; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int n = n_t * BLOCK_N + 8 * j + 2 * (lane & 3) + e;
+                if (n >= N) continue;
+                float f = acc[mh * (BLOCK_N / 2) + 4 * j + 2 * h + e];
+                if (p.bias) f += p.bias[n];
+                if (p.addend) f += __bfloat162float(p.addend[opix * p.ldc + n]);
+                orow[n] = __float2bfloat16_rn(f);
+              }
           }
-        }
-      }
       }
     }
   }
@@ -1008,8 +1025,7 @@ static void fill_taps(TapEntry* taps, int R, int S, int cin) {
 
 static int pick_block_n(long long m_tiles, int n) {
   // favour wide tiles (fewer re-reads of the activation tile), but keep the last wave full.  128 is the widest tile:
-  // a warpgroup holds its 64 x BLOCK_N fp32 accumulators in registers, and the 128 x BLOCK_N exchange tile plus four
-  // 32 KB stages fill the 227 KB of shared memory.
+  // a consumer warpgroup holds the whole 128 x BLOCK_N tile in fp32 registers (128 per thread at BLOCK_N = 128).
   const int sms = sm_count();
   int best = 64; double best_score = -1;
   const int cands[2] = {128, 64};
@@ -1029,7 +1045,7 @@ constexpr int kSmemMax = 232448;                 // 227 KB: the per-CTA opt-in l
 
 template <int BN, bool MULTI, bool BNB = false>
 static int launch_fwd(const AMaps& a, const CUtensorMap& b, FwdParams& p, cudaStream_t st) {
-  constexpr int smem = fwd_stages(BN) * (kBlockM * kBlockK * 2 + BN * kBlockK * 2) + fwd_tail(BN);
+  constexpr int smem = fwd_smem(BN);
   static_assert(smem <= kSmemMax, "fwd smem budget");
   const int n_tiles = (p.N + BN - 1) / BN;
   static bool attr_set = false;
@@ -1047,7 +1063,7 @@ static int launch_fwd(const AMaps& a, const CUtensorMap& b, FwdParams& p, cudaSt
   }
   if (ctiles > 0x7fffffffll || ctiles <= 0) return TP_ERR_UNSUPPORTED;
   const int grid = (int)(ctiles < sm_count() ? ctiles : sm_count());
-  TP_CUDA_CHECK(launch(k_igemm_fwd<BN, MULTI, BNB>, dim3(grid), dim3(kThreads), (size_t)smem, st, a, b, p));
+  TP_CUDA_CHECK(launch(k_igemm_fwd<BN, MULTI, BNB>, dim3(grid), dim3(kFwdThreads), (size_t)smem, st, a, b, p));
   TP_LAUNCH_CHECK();
   return TP_OK;
 }
