@@ -34,7 +34,7 @@ extern "C" {
 
 const char* tp_strerror(int code);
 const char* tp_last_cuda_error(void);      /* text of the last CUDA error seen by this thread */
-int         tp_abi_version(void);          /* bumps when a signature changes */
+int         tp_abi_version(void);          /* bumps when a signature changes; 9: tp_cifar_augment takes idx */
 int         tp_device_sm_count(void);      /* cached multiprocessor count of the current device */
 /* Programmatic dependent launch for the train-step kernels (default off; TP_PDL=1 in the environment turns it on).
  * Returns the previous setting.  A debugging / A-B switch: results are bit-identical either way. */
@@ -155,12 +155,16 @@ int tp_im2col_stem(const void* src, int src_dtype, int64_t sn, int64_t sc, int64
 
 /* ---- data path either side of the model (SURVEY.md §8(f) row 3) --------------------------
  * tp_cifar_augment: random translate (batch_crop of the reflect-padded images, utils/dataset.py:43-69), per-image
- * left-right flip (:38-40) and cutout (:72-98) of CifarLoader.__iter__ (:192-226) as ONE gather pass:
- *   out[n][c][y][x] = inside_cut(n,y,x) ? 0 : src[n][c][y + r + shifts[n][0]][xf + r + shifts[n][1]],  xf = flip[n] ? w-1-x : x
- * src fp32 [n][c][h+2r][w+2r] contiguous, out fp32 [n][c][h][w]; shifts int64 [n][2] in [-r, r] (NULL: no translate, then
- * r must describe the padding actually present, usually 0), flip uint8 [n] (NULL: none), cut_y / cut_x int64 [n] top-left
- * corners of a cut_size square (both NULL: none).  The draws are the caller's (torch RNG, reference order). */
-int tp_cifar_augment(const void* src, void* out, const int64_t* shifts, const uint8_t* flip,
+ * left-right flip (:38-40) and cutout (:72-98) of CifarLoader.__iter__ (:192-226) as ONE gather pass, optionally fused with
+ * the batch gather images[idx] (:224-226):
+ *   out[j][c][y][x] = inside_cut(s,y,x) ? 0 : src[s][c][y + r + shifts[s][0]][xf + r + shifts[s][1]],  xf = flip[s] ? w-1-x : x,
+ *   s = idx ? idx[j] : j
+ * src fp32 [N][c][h+2r][w+2r] contiguous, out fp32 [n][c][h][w]; idx int64 [n] source images in [0, N), repeats allowed
+ * (NULL: s = j and N = n).  The draws are per SOURCE image, as the reference draws them over the whole data set before
+ * it permutes: shifts int64 [N][2] in [-r, r] (NULL: no translate, then r must describe the padding actually present,
+ * usually 0), flip uint8 [N] (NULL: none), cut_y / cut_x int64 [N] top-left corners of a cut_size square (both NULL:
+ * none).  The draws are the caller's (torch RNG, reference order). */
+int tp_cifar_augment(const void* src, void* out, const int64_t* idx, const int64_t* shifts, const uint8_t* flip,
                      const int64_t* cut_y, const int64_t* cut_x, int cut_size,
                      int n, int c, int h, int w, int r, void* stream);
 /* Synthetic batches (stand-in for the FFCV / CIFAR loaders, which need data sets): Philox4x32-10, counter

@@ -4,7 +4,8 @@
 //                     (utils/dataset.py:192-226): random translate = batch_crop of the reflect-padded images (:43-69),
 //                     per-image left-right flip (:38-40) and cutout (:72-98), fused into ONE gather pass — the
 //                     reference runs a masked-assignment loop over 2(2r+1) shifts, a where() and a masked_fill(), each a
-//                     full pass.  The random draws (shifts, flip mask, cutout corners) stay torch's: their RNG stream is
+//                     full pass.  With a source index it is also the batch gather (images[perm[slice]]), so an epoch
+//                     never writes a whole augmented copy of the data set.  The random draws (shifts, flip mask, cutout corners) stay torch's: their RNG stream is
 //                     part of the parity contract, exactly like set_er_mask.
 //   k_synth_normal / k_synth_labels : the synthetic on-device generator standing in for FFCV / the CIFAR tensors
 //                     (no data sets here): counter-based Philox4x32-10 -> Box-Muller, four values per counter, written
@@ -14,9 +15,11 @@
 
 namespace tp {
 
-// out[n][c][y][x] = cut(n, y, x) ? 0 : src[n][c][y + r + sy[n]][xf + r + sx[n]],  xf = flip[n] ? W-1-x : x
-// src is [N][C][H+2r][W+2r] (r = 0 and no shifts: plain flip / cutout); every array of draws is optional.
+// out[n][c][y][x] = cut(s, y, x) ? 0 : src[s][c][y + r + sy[s]][xf + r + sx[s]],  xf = flip[s] ? W-1-x : x,
+// s = idx ? idx[n] : n.  src is [N_src][C][H+2r][W+2r] (r = 0 and no shifts: plain flip / cutout); every array of draws is
+// optional and, like the reference's whole-dataset draws, indexed by the SOURCE image.
 __global__ void __launch_bounds__(256) k_cifar_augment(const float* __restrict__ src, float* __restrict__ out,
+                                                       const long long* __restrict__ idx,
                                                        const long long* __restrict__ shifts, const unsigned char* __restrict__ flip,
                                                        const long long* __restrict__ cut_y, const long long* __restrict__ cut_x,
                                                        int cut_size, int N, int C, int H, int W, int r) {
@@ -26,16 +29,17 @@ __global__ void __launch_bounds__(256) k_cifar_augment(const float* __restrict__
     const int x = (int)(i % W); long long t = i / W;
     const int y = (int)(t % H); t /= H;
     const int c = (int)(t % C); const int n = (int)(t / C);
+    const long long s = idx ? idx[n] : (long long)n;
     float v = 0.f;
     bool cut = false;
     if (cut_y) {
-      const long long dy = y - cut_y[n], dx = x - cut_x[n];
+      const long long dy = y - cut_y[s], dx = x - cut_x[s];
       cut = dy >= 0 && dy < cut_size && dx >= 0 && dx < cut_size;
     }
     if (!cut) {
-      const int sy = shifts ? (int)shifts[2 * n] : 0, sx = shifts ? (int)shifts[2 * n + 1] : 0;
-      const int xf = (flip && flip[n]) ? W - 1 - x : x;
-      v = src[(((long long)n * C + c) * Hp + (y + r + sy)) * Wp + (xf + r + sx)];
+      const int sy = shifts ? (int)shifts[2 * s] : 0, sx = shifts ? (int)shifts[2 * s + 1] : 0;
+      const int xf = (flip && flip[s]) ? W - 1 - x : x;
+      v = src[((s * C + c) * Hp + (y + r + sy)) * Wp + (xf + r + sx)];
     }
     out[i] = v;
   }
@@ -103,7 +107,7 @@ using namespace tp;
 
 extern "C" {
 
-int tp_cifar_augment(const void* src, void* out, const int64_t* shifts, const uint8_t* flip,
+int tp_cifar_augment(const void* src, void* out, const int64_t* idx, const int64_t* shifts, const uint8_t* flip,
                      const int64_t* cut_y, const int64_t* cut_x, int cut_size,
                      int n, int c, int h, int w, int r, void* stream) {
   if (!src || !out || n <= 0 || c <= 0 || h <= 0 || w <= 0 || r < 0) return TP_ERR_INVALID;
@@ -112,7 +116,7 @@ int tp_cifar_augment(const void* src, void* out, const int64_t* shifts, const ui
   const long long total = (long long)n * c * h * w;
   const long long g = (total + 255) / 256, gm = (long long)sm_count() * 16;
   k_cifar_augment<<<(unsigned)(g < gm ? g : gm), 256, 0, (cudaStream_t)stream>>>(
-      (const float*)src, (float*)out, (const long long*)shifts, (const unsigned char*)flip,
+      (const float*)src, (float*)out, (const long long*)idx, (const long long*)shifts, (const unsigned char*)flip,
       (const long long*)cut_y, (const long long*)cut_x, cut_size, n, c, h, w, r);
   TP_LAUNCH_CHECK();
   return TP_OK;

@@ -3,11 +3,14 @@
 ``PruningHarness(cfg, gpu_id, expt_dir, model=None)`` and ``.train_one_level(epochs_per_level, level)`` keep the
 reference's behaviour (:28-50, :159-269): a fresh optimizer and LR schedule per level (momentum never carries
 over), ``model_init.pt`` / ``optimizer_init.pt`` at level 0, ``model_rewind.pt`` at ``pruning_params.rewind_epoch``,
-per-level CSV + summary CSV.  Optimizer = ``FusedSGD`` (same state-dict layout as torch.optim.SGD), loaders = the
-synthetic on-device generator (the real loaders are out of scope).
+per-level CSV + summary CSV.  Optimizer = ``FusedSGD`` (same state-dict layout as torch.optim.SGD).  Loaders: the
+reference's device-resident CIFAR loader (``AirbenchLoaders``) when a CIFAR config names a ``dataset_params.dataloader_type``
+other than ``synthetic`` (the reference's ``dp_cifar*.yaml`` say ``torch``); otherwise, and for ImageNet (FFCV /
+WebDataset are out of scope), the synthetic on-device generator.
 """
 import csv
 import os
+import sys
 from typing import Optional
 
 import torch
@@ -16,7 +19,7 @@ import torch.nn as nn
 from ..optim import FusedSGD
 from ..utils import schedulers
 from ..utils.custom_models import CustomModel, TorchVisionModel
-from ..utils.dataset import SyntheticLoaders
+from ..utils.dataset import AirbenchLoaders, SyntheticLoaders
 from ..utils.harness_utils import save_model
 from .base_harness import BaseHarness
 
@@ -42,9 +45,16 @@ class PruningHarness(BaseHarness):
         return model
 
     def _setup_dataloaders(self):
-        world = torch.distributed.get_world_size() if self.distributed else 1
-        rank = torch.distributed.get_rank() if self.distributed else 0
-        loaders = SyntheticLoaders(self.cfg, self.device, world, rank)
+        kind = getattr(self.cfg.dataset_params, "dataloader_type", None)
+        if self.dataset_name.startswith("cifar") and kind is not None and kind != "synthetic":
+            loaders = AirbenchLoaders(self.cfg, self.device)          # reference :145-148; CIFAR never runs distributed
+            print(f"Data: CifarLoader ({self.cfg.dataset_params.dataset_name}, {self.cfg.dataset_params.data_root_dir})",
+                  file=sys.stderr)
+        else:
+            world = torch.distributed.get_world_size() if self.distributed else 1
+            rank = torch.distributed.get_rank() if self.distributed else 0
+            loaders = SyntheticLoaders(self.cfg, self.device, world, rank)
+            print(f"Data: SyntheticLoaders ({self.cfg.dataset_params.dataset_name}-shaped on-device batches)", file=sys.stderr)
         return loaders.train_loader, loaders.test_loader
 
     def _setup_optimizer(self):
