@@ -34,7 +34,7 @@ extern "C" {
 
 const char* tp_strerror(int code);
 const char* tp_last_cuda_error(void);      /* text of the last CUDA error seen by this thread */
-int         tp_abi_version(void);          /* bumps when a signature changes; 9: tp_cifar_augment takes idx */
+int         tp_abi_version(void);          /* bumps when a signature changes; 9: tp_cifar_augment takes idx; 10: tp_resized_crop */
 int         tp_device_sm_count(void);      /* cached multiprocessor count of the current device */
 /* Programmatic dependent launch for the train-step kernels (default off; TP_PDL=1 in the environment turns it on).
  * Returns the previous setting.  A debugging / A-B switch: results are bit-identical either way. */
@@ -167,6 +167,25 @@ int tp_im2col_stem(const void* src, int src_dtype, int64_t sn, int64_t sc, int64
 int tp_cifar_augment(const void* src, void* out, const int64_t* idx, const int64_t* shifts, const uint8_t* flip,
                      const int64_t* cut_y, const int64_t* cut_x, int cut_size,
                      int n, int c, int h, int w, int r, void* stream);
+/* tp_resized_crop: the ImageNet loader's RandomResizedCrop / centre crop + RandomHorizontalFlip + NormalizeImage
+ * (utils/dataset.py:384-400, what FFCV's decoders and transforms hand the model) for a whole batch in ONE launch:
+ *   out[b][c][y][x] = (R_b[c][y][xf] - mean255[c]) / std255[c],  xf = flip ? size-1-x : x,
+ * R_b = the box rows [top, top+h) x columns [left, left+w) of table[b].src alone, resized to size x size with PIL's
+ * bilinear filter: F.interpolate(box, (size, size), mode="bilinear", antialias=True, align_corners=False), i.e. the
+ * separable triangle filter of half-width max(in/out, 1), taps clamped to the box, normalised per output pixel.
+ * table: device array of n entries (n <= 65535); src uint8 [3][H][W] contiguous (CHW RGB); the box must lie inside the
+ * image (h, w >= 1) and be at most 1023 * size wide, else that image's output is NaN.  out fp32 [n][size][size][3]
+ * (logical [n][3][size][size] with channels_last strides); size in [1, 2048].  mean255 / std255: host arrays of 3
+ * (NULL: 0 / 1).  Accumulation is fp32; a box of exactly size x size reproduces (v - mean255) / std255 bit for bit. */
+typedef struct tp_crop_entry {
+  const void* src;               /* uint8 [3][H][W], device memory */
+  int32_t H, W;                  /* image extents */
+  int32_t top, left, h, w;       /* crop box */
+  int32_t flip;                  /* != 0: mirror the output left-right */
+  int32_t reserved;              /* 0 */
+} tp_crop_entry;
+int tp_resized_crop(const tp_crop_entry* table, int n, int size, const float* mean255, const float* std255, void* out,
+                    void* stream);
 /* Synthetic batches (stand-in for the FFCV / CIFAR loaders, which need data sets): Philox4x32-10, counter
  * (counter_offset + i/4, 0, 0, 0), key = seed; element i takes word i%4.  tp_synth_normal writes N(0,1) fp32 (Box-Muller
  * on 24-bit uniforms; raw_words != 0: the 32-bit words themselves, for bit-exact pinning of the stream);

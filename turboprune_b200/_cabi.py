@@ -27,6 +27,10 @@ class StageItem(ctypes.Structure):
                [("kmask_f", c_void_p), ("kmask_d", c_void_p)]
 
 
+class CropEntry(ctypes.Structure):
+    _fields_ = [("src", c_void_p)] + [(n, c_int32) for n in ("H", "W", "top", "left", "h", "w", "flip", "reserved")]
+
+
 # name -> (restype, argtypes); every symbol the header declares
 SIGNATURES = {
     "tp_strerror": (c_char_p, [c_int]),
@@ -55,6 +59,7 @@ SIGNATURES = {
     "tp_im2col_c8": (c_int, [c_void_p] + [c_int] * 11 + [c_void_p, c_int, c_void_p]),
     "tp_im2col_stem": (c_int, [c_void_p, c_int, c_int64, c_int64, c_int64, c_int64] + [c_int] * 13 + [c_void_p, c_int, c_void_p]),
     "tp_cifar_augment": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "tp_resized_crop": (c_int, [c_void_p, c_int, c_int, POINTER(c_float), POINTER(c_float), c_void_p, c_void_p]),
     "tp_synth_normal": (c_int, [c_void_p, c_int64, c_uint64, c_uint64, c_int, c_void_p]),
     "tp_synth_labels": (c_int, [c_void_p, c_int64, c_int, c_uint64, c_uint64, c_void_p]),
     "tp_conv_workspace_bytes": (c_size_t, [POINTER(ConvDesc), c_int]),

@@ -5,8 +5,9 @@ reference's behaviour (:28-50, :159-269): a fresh optimizer and LR schedule per 
 over), ``model_init.pt`` / ``optimizer_init.pt`` at level 0, ``model_rewind.pt`` at ``pruning_params.rewind_epoch``,
 per-level CSV + summary CSV.  Optimizer = ``FusedSGD`` (same state-dict layout as torch.optim.SGD).  Loaders: the
 reference's device-resident CIFAR loader (``AirbenchLoaders``) when a CIFAR config names a ``dataset_params.dataloader_type``
-other than ``synthetic`` (the reference's ``dp_cifar*.yaml`` say ``torch``); otherwise, and for ImageNet (FFCV /
-WebDataset are out of scope), the synthetic on-device generator.
+other than ``synthetic`` (the reference's ``dp_cifar*.yaml`` say ``torch``); ``ImageFolderImagenet`` (GPU-decoded
+ImageFolder tree) when an ImageNet config says ``dataloader_type: imagefolder``; otherwise (FFCV / WebDataset are out of
+scope) the synthetic on-device generator.
 """
 import csv
 import os
@@ -19,7 +20,7 @@ import torch.nn as nn
 from ..optim import FusedSGD
 from ..utils import schedulers
 from ..utils.custom_models import CustomModel, TorchVisionModel
-from ..utils.dataset import AirbenchLoaders, SyntheticLoaders
+from ..utils.dataset import AirbenchLoaders, ImageFolderImagenet, SyntheticLoaders
 from ..utils.harness_utils import save_model
 from .base_harness import BaseHarness
 
@@ -46,13 +47,17 @@ class PruningHarness(BaseHarness):
 
     def _setup_dataloaders(self):
         kind = getattr(self.cfg.dataset_params, "dataloader_type", None)
+        world = torch.distributed.get_world_size() if self.distributed else 1
+        rank = torch.distributed.get_rank() if self.distributed else 0
         if self.dataset_name.startswith("cifar") and kind is not None and kind != "synthetic":
             loaders = AirbenchLoaders(self.cfg, self.device)          # reference :145-148; CIFAR never runs distributed
             print(f"Data: CifarLoader ({self.cfg.dataset_params.dataset_name}, {self.cfg.dataset_params.data_root_dir})",
                   file=sys.stderr)
+        elif self.dataset_name.startswith("imagenet") and kind == "imagefolder":
+            loaders = ImageFolderImagenet(self.cfg, self.device, world, rank)
+            print(f"Data: ImageFolderImagenet ({self.cfg.dataset_params.data_root_dir}/{{train,val}}, rank {rank} of {world})",
+                  file=sys.stderr)
         else:
-            world = torch.distributed.get_world_size() if self.distributed else 1
-            rank = torch.distributed.get_rank() if self.distributed else 0
             loaders = SyntheticLoaders(self.cfg, self.device, world, rank)
             print(f"Data: SyntheticLoaders ({self.cfg.dataset_params.dataset_name}-shaped on-device batches)", file=sys.stderr)
         return loaders.train_loader, loaders.test_loader

@@ -4,8 +4,12 @@
   arguments, random draws and batches.  The data set lives on the GPU; each batch is ONE ``tp_cifar_augment`` launch
   that gathers the permuted source images and applies the epoch's translate / flip / cutout on the way, so an epoch
   never writes an augmented copy of the whole data set and never waits on the host.
-* ``SyntheticLoaders``: the on-device generator standing in for loaders whose data is not at hand (ImageNet's FFCV /
-  WebDataset loaders, :347-546, are out of scope; benchmarks and synthetic configs use it for every data set).
+* ``ImageFolderLoader`` / ``ImageFolderImagenet``: ImageNet from the standard ImageFolder tree
+  ``{root}/{train,val}/<wnid>/*.JPEG`` with the transforms of the reference's FFCV pipelines (:347-430): files read by a
+  thread pool, decoded batched on the GPU (nvjpeg through torchvision), and every batch's crops resized, mirrored and
+  normalised by ONE ``tp_resized_crop`` launch, prepared on a side stream while the caller trains on the previous batch.
+* ``SyntheticLoaders``: the on-device generator standing in for loaders whose data is not at hand (the FFCV beton and
+  WebDataset readers, :347-546, are out of scope; benchmarks and synthetic configs use it for every data set).
 
 Same batch contract throughout: an iterable of ``(images fp32 [B,3,H,W], labels int64 [B])`` with ``len()``;
 ImageNet-shaped synthetic batches come channels_last like FFCV's ToTorchImage.  Synthetic loaders are seeded per rank;
@@ -13,10 +17,17 @@ either a fixed number of distinct batches is generated once and cycled (an epoch
 (``dataset_params.synthetic_fresh``) every step draws a new batch on the device.  ``DevicePrefetcher`` is the
 host->device leg for loaders that produce pinned host batches.
 """
+import math
 import os
-from ctypes import c_void_p
+import queue
+import sys
+import threading
+from concurrent.futures import ThreadPoolExecutor
+from ctypes import c_float, c_void_p, sizeof
+from functools import lru_cache
 from math import ceil
 
+import numpy as np
 import torch
 
 from .. import _cabi, ops
@@ -342,3 +353,305 @@ class AirbenchLoaders:
                                         aug={"flip": True, "translate": 2}, altflip=True, dataset=dp.dataset_name, device=device)
         self.test_loader = CifarLoader(path=dp.data_root_dir, batch_size=dp.total_batch_size, train=False,
                                        dataset=dp.dataset_name, device=device)
+
+
+# ---- ImageNet from an ImageFolder tree (reference utils/dataset.py:347-430 reads FFCV betons written from it) ----------
+IMAGENET_MEAN = tuple(v * 255 for v in (0.485, 0.456, 0.406))     # reference :28-29, already scaled to 0..255
+IMAGENET_STD = tuple(v * 255 for v in (0.229, 0.224, 0.225))
+DEFAULT_CROP_RATIO = 224 / 256
+
+
+def resized_crop(images, boxes, flips, size=224, mean=IMAGENET_MEAN, std=IMAGENET_STD):
+    """One ``tp_resized_crop`` launch on the current stream.  ``images``: list of uint8 [3, H, W] contiguous CUDA
+    tensors; ``boxes``: int [B, 4] (top, left, h, w) per image, inside it; ``flips``: bool [B].  Returns fp32
+    [B, 3, size, size] with channels_last strides: each box resized like
+    ``F.interpolate(box, (size, size), mode="bilinear", antialias=True)``, mirrored where flipped, then
+    ``(v - mean) / std``."""
+    if not images or not images[0].is_cuda:
+        raise RuntimeError("turboprune_b200 resized_crop needs CUDA images (H100 / sm_90a); there is no CPU path")
+    dev, n = images[0].device, len(images)
+    boxes, flips = torch.as_tensor(boxes).tolist(), torch.as_tensor(flips).tolist()
+    if len(boxes) != n or len(flips) != n:
+        raise ValueError("resized_crop: one box and one flip per image")
+    table = torch.empty(n * sizeof(_cabi.CropEntry), dtype=torch.uint8, pin_memory=True)
+    entries = (_cabi.CropEntry * n).from_address(table.data_ptr())
+    for i, (img, (t, l, h, w), f) in enumerate(zip(images, boxes, flips)):
+        if img.dtype != torch.uint8 or img.dim() != 3 or img.shape[0] != 3 or not img.is_contiguous() or img.device != dev:
+            raise ValueError(f"resized_crop: image {i} must be uint8 [3, H, W] contiguous on {dev}")
+        H, W = img.shape[1:]
+        if not (h >= 1 and w >= 1 and 0 <= t and t + h <= H and 0 <= l and l + w <= W and w <= 1023 * size):
+            raise ValueError(f"resized_crop: box {(t, l, h, w)} of image {i} does not fit its {H} x {W} image")
+        entries[i] = _cabi.CropEntry(img.data_ptr(), H, W, t, l, h, w, int(bool(f)), 0)
+    dtab = table.to(dev, non_blocking=True)
+    out = torch.empty(n, size, size, 3, dtype=torch.float32, device=dev)
+    lib = _cabi.load()
+    with torch.cuda.device(dev):
+        rc = lib.tp_resized_crop(_ptr(dtab), n, int(size), (c_float * 3)(*mean), (c_float * 3)(*std), _ptr(out),
+                                 _cabi.stream_ptr(dev))
+    _cabi.check(rc, "tp_resized_crop")
+    ops._count()
+    return out.permute(0, 3, 1, 2)
+
+
+def random_resized_crop_boxes(hw, u_area, u_ratio, u_off, scale=(0.08, 1.0), ratio=(3 / 4, 4 / 3)):
+    """torchvision's / FFCV's ``RandomResizedCrop`` box draw, vectorised over images, from pre-drawn uniforms in [0, 1):
+    ``hw`` int [B, 2] image extents, ``u_area`` / ``u_ratio`` float64 [B, 10] (one pair per attempt), ``u_off`` float64
+    [B, 2].  Attempt k: area = H*W*U(scale), aspect = exp(U(log ratio)), w = round(sqrt(area*aspect)),
+    h = round(sqrt(area/aspect)); the first attempt with 0 < w <= W and 0 < h <= H wins and is placed at a uniform
+    offset; without one, the ratio-clamped centre crop.  Returns int64 [B, 4] (top, left, h, w)."""
+    hw = torch.as_tensor(hw, dtype=torch.float64)
+    H, W = hw[:, :1], hw[:, 1:]
+    target = H * W * (scale[0] + (scale[1] - scale[0]) * u_area)
+    lr0, lr1 = math.log(ratio[0]), math.log(ratio[1])
+    ar = torch.exp(lr0 + (lr1 - lr0) * u_ratio)
+    w = torch.round(torch.sqrt(target * ar))
+    h = torch.round(torch.sqrt(target / ar))
+    ok = (w > 0) & (w <= W) & (h > 0) & (h <= H)
+    k = ok.to(torch.int8).argmax(1, keepdim=True)                  # first accepted attempt (0 when none is)
+    hit = ok.any(1)
+    H, W = H.squeeze(1), W.squeeze(1)
+    w, h = w.gather(1, k).squeeze(1), h.gather(1, k).squeeze(1)
+    top = torch.minimum(torch.floor(u_off[:, 0] * (H - h + 1)), H - h)
+    left = torch.minimum(torch.floor(u_off[:, 1] * (W - w + 1)), W - w)
+    in_ratio = W / H
+    tall, wide = in_ratio < min(ratio), in_ratio > max(ratio)
+    fw = torch.where(wide, torch.round(H * max(ratio)), W)
+    fh = torch.where(tall, torch.round(W / min(ratio)), H)
+    box = torch.stack([torch.where(hit, top, torch.div(H - fh, 2, rounding_mode="floor")),
+                       torch.where(hit, left, torch.div(W - fw, 2, rounding_mode="floor")),
+                       torch.where(hit, h, fh), torch.where(hit, w, fw)], 1)
+    return box.to(torch.int64)
+
+
+def center_crop_box(H, W, ratio=DEFAULT_CROP_RATIO):
+    """FFCV's ``CenterCropRGBImageDecoder`` box: a c x c square, c = int(ratio * min(H, W)) (at least 1), centred."""
+    c = max(1, int(ratio * min(H, W)))
+    return (H - c) // 2, (W - c) // 2, c, c
+
+
+@lru_cache(maxsize=4)
+def scan_image_folder(root):
+    """``torchvision.datasets.ImageFolder``'s index of ``root``: sorted class directories give class i, files in its
+    order.  Returns (classes, relative paths as a bytes array, labels int64 array); cached per root."""
+    from torchvision.datasets.folder import IMG_EXTENSIONS, find_classes, make_dataset
+    classes, to_idx = find_classes(root)
+    samples = make_dataset(root, to_idx, IMG_EXTENSIONS)
+    if not samples:
+        raise FileNotFoundError(f"ImageFolderLoader: no images under {root}")
+    rel = np.array([os.fsencode(os.path.relpath(p, root)) for p, _ in samples])
+    return tuple(classes), rel, np.array([c for _, c in samples], dtype=np.int64)
+
+
+def _jpeg_components(data):
+    """Number of colour components from the first SOF marker of JPEG bytes (uint8 tensor); None if it is not a JPEG
+    nvjpeg can be handed (no SOI, or no frame header found)."""
+    b = data[:65536].numpy().tobytes()
+    if len(b) < 4 or b[0] != 0xFF or b[1] != 0xD8:
+        return None
+    i = 2
+    while i + 9 < len(b):
+        if b[i] != 0xFF:
+            return None
+        m = b[i + 1]
+        if m == 0xFF:
+            i += 1
+            continue
+        if 0xC0 <= m <= 0xCF and m not in (0xC4, 0xC8, 0xCC):
+            return b[i + 9]
+        if m in (0xD8, 0x01) or 0xD0 <= m <= 0xD7:
+            i += 2
+            continue
+        i += 2 + (b[i + 2] << 8 | b[i + 3])
+    return None
+
+
+_warned_files = set()
+
+
+def decode_images(datas, device, names=None):
+    """Raw file bytes (uint8 CPU tensors) -> list of uint8 [3, H, W] RGB tensors on ``device``, plus a bool per image
+    telling whether it went through the CPU.  JPEGs with 1 or 3 components are decoded by nvjpeg in one batched call;
+    what nvjpeg cannot take (CMYK, PNG or other data named .JPEG, a file the batched call rejects) is decoded by
+    torchvision's CPU ``decode_image`` and uploaded.  A file no decoder accepts becomes a mean-coloured 8 x 8 image,
+    with a warning, so that one bad file never fails a batch."""
+    from torchvision.io import ImageReadMode, decode_image, decode_jpeg
+    out, on_cpu = [None] * len(datas), [False] * len(datas)
+    gpu = [i for i, d in enumerate(datas) if _jpeg_components(d) in (1, 3)]
+    if gpu:
+        try:
+            dec = decode_jpeg([datas[i] for i in gpu], mode=ImageReadMode.RGB, device=device)
+        except RuntimeError:
+            dec = []
+            for i in gpu:
+                try:
+                    dec.append(decode_jpeg(datas[i], mode=ImageReadMode.RGB, device=device))
+                except RuntimeError:
+                    dec.append(None)
+        for i, x in zip(gpu, dec):
+            if x is not None and x.dim() == 3 and x.shape[0] == 3:
+                out[i] = x.contiguous()
+    for i, x in enumerate(out):
+        if x is not None:
+            continue
+        on_cpu[i] = True
+        try:
+            x = decode_image(datas[i], mode=ImageReadMode.RGB)
+        except RuntimeError:
+            name = names[i] if names is not None else i
+            if name not in _warned_files:
+                _warned_files.add(name)
+                print(f"ImageFolderLoader: cannot decode {name}; using a blank image", file=sys.stderr)
+            x = torch.tensor([round(m) for m in IMAGENET_MEAN], dtype=torch.uint8).view(3, 1, 1).expand(3, 8, 8)
+        out[i] = x.contiguous().pin_memory().to(device, non_blocking=True)
+    return out, on_cpu
+
+
+def _read_file(path):
+    with open(path, "rb") as f:
+        return torch.frombuffer(bytearray(f.read()), dtype=torch.uint8)
+
+
+class ImageFolderLoader:
+    """One split of an ImageFolder tree as an iterable of ``(images fp32 [B, 3, S, S] channels_last, labels int64 [B])``
+    on ``device``, B = ``total_batch_size // world_size``: the batch contract of the reference's FFCV loaders
+    (utils/dataset.py:380-430).
+
+    ``train=True``: every epoch one permutation seeded by ``(seed, epoch)``, the same on every rank; global batch g is
+    ``perm[g*T:(g+1)*T]`` (T = total_batch_size) and rank r takes its r-th slice of B; ``drop_last``, so
+    ``len() = N // T``.  Each image gets a RandomResizedCrop(S, scale=(0.08, 1), ratio=(3/4, 4/3)) box and a flip with
+    p = 0.5, drawn on the host from the same generator for the whole global batch (a sample's draws do not depend on the
+    world size).  ``train=False``: images ``i % world_size == rank`` in order, FFCV's centre crop (ratio 224/256), no
+    flip, the last partial batch kept, so the ranks' counts add up to the whole split.
+
+    Batch i+1 is read (``num_workers`` threads), decoded and cropped on a side stream by a producer thread while the
+    caller uses batch i; the caller's stream waits on an event before it sees a batch, and ``record_stream`` keeps each
+    batch alive until the caller's work on it is done.  ``last_indices`` / ``last_boxes`` / ``last_flips`` describe the
+    batch last handed out (sample indices into ``labels``, (top, left, h, w) per image, mirrored or not)."""
+
+    def __init__(self, root, train, total_batch_size, device=None, num_workers=8, seed=0, world_size=1, rank=0,
+                 size=224):
+        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+        if self.device.type != "cuda":
+            raise RuntimeError("turboprune_b200 ImageFolderLoader decodes and crops on a CUDA device (H100 / sm_90a)")
+        if not 0 <= rank < world_size or total_batch_size < world_size:
+            raise ValueError(f"ImageFolderLoader: rank {rank} of {world_size} with total batch {total_batch_size}")
+        self.root, self.train, self.size = os.fspath(root), bool(train), int(size)
+        self.classes, self.paths, self.labels = scan_image_folder(self.root)
+        self.total_batch_size, self.batch_size = int(total_batch_size), int(total_batch_size) // world_size
+        self.world_size, self.rank, self.seed = world_size, rank, int(seed)
+        self.num_workers = max(1, int(num_workers))
+        self.epoch = 0
+        self.last_indices = self.last_boxes = self.last_flips = None
+
+    def __len__(self):
+        n = len(self.labels)
+        if self.train:
+            return n // self.total_batch_size
+        return ceil(len(range(self.rank, n, self.world_size)) / self.batch_size)
+
+    def _plan(self, epoch):
+        """Per batch: (sample indices [B], uniforms for this rank's slice or None)."""
+        n, B = len(self.labels), self.batch_size
+        if not self.train:
+            idx = torch.arange(self.rank, n, self.world_size)
+            for i in range(len(self)):
+                yield idx[i * B:(i + 1) * B], None
+            return
+        g = torch.Generator().manual_seed(((self.seed << 32) + epoch) & (2 ** 64 - 1))
+        perm, T = torch.randperm(n, generator=g), self.total_batch_size
+        s = slice(self.rank * B, (self.rank + 1) * B)
+        for i in range(len(self)):
+            u = [torch.rand(T, k, generator=g, dtype=torch.float64)[s] for k in (10, 10, 2, 1)]
+            yield perm[i * T:(i + 1) * T][s], u
+
+    def _batch(self, idx, u, datas):
+        """Decode, draw the boxes, one crop launch, labels: all on the current (side) stream."""
+        names = [self.paths[i] for i in idx.tolist()]
+        images, _ = decode_images(datas, self.device, names)
+        cur = torch.cuda.current_stream(self.device)
+        for x in images:
+            x.record_stream(cur)          # nvjpeg may allocate on its own stream; the crop reads on this one
+        hw = torch.tensor([x.shape[1:] for x in images], dtype=torch.int64)
+        if u is None:
+            boxes = torch.tensor([center_crop_box(h, w) for h, w in hw.tolist()], dtype=torch.int64)
+            flips = torch.zeros(len(images), dtype=torch.bool)
+        else:
+            boxes = random_resized_crop_boxes(hw, u[0], u[1], u[2])
+            flips = u[3][:, 0] < 0.5
+        x = resized_crop(images, boxes, flips, self.size)
+        y = torch.from_numpy(self.labels[idx.numpy()]).pin_memory().to(self.device, non_blocking=True)
+        return x, y, (idx, boxes, flips)
+
+    def _produce(self, epoch, q, stop):
+        try:
+            side = torch.cuda.Stream(self.device)
+            with ThreadPoolExecutor(self.num_workers) as pool, torch.cuda.device(self.device), torch.cuda.stream(side):
+                read = lambda idx: [pool.submit(_read_file, os.path.join(self.root, os.fsdecode(self.paths[i])))
+                                    for i in idx.tolist()]
+                plan = self._plan(epoch)
+                nxt = next(plan, None)
+                pending = read(nxt[0]) if nxt is not None else None
+                while nxt is not None and not stop.is_set():
+                    idx, u = nxt
+                    nxt = next(plan, None)
+                    datas = [f.result() for f in pending]
+                    pending = read(nxt[0]) if nxt is not None else None      # the next batch's files meanwhile
+                    x, y, meta = self._batch(idx, u, datas)
+                    ev = torch.cuda.Event()
+                    ev.record(side)
+                    item = (x, y, ev, meta)
+                    while not stop.is_set():
+                        try:
+                            q.put(item, timeout=0.1)
+                            break
+                        except queue.Full:
+                            pass
+                if pending is not None:
+                    for f in pending:
+                        f.cancel()
+        except BaseException as e:               # handed to the consumer, which raises it
+            q.put(e)
+            return
+        q.put(None)
+
+    def __iter__(self):
+        epoch = self.epoch
+        self.epoch += 1
+        q, stop = queue.Queue(maxsize=1), threading.Event()
+        worker = threading.Thread(target=self._produce, args=(epoch, q, stop), daemon=True,
+                                  name=f"ImageFolderLoader-{'train' if self.train else 'val'}")
+        worker.start()
+        try:
+            while True:
+                item = q.get()
+                if item is None:
+                    return
+                if isinstance(item, BaseException):
+                    raise item
+                x, y, ev, meta = item
+                cur = torch.cuda.current_stream(self.device)
+                cur.wait_event(ev)
+                x.record_stream(cur); y.record_stream(cur)
+                self.last_indices, self.last_boxes, self.last_flips = meta
+                yield x, y
+        finally:
+            stop.set()
+            while worker.is_alive():
+                try:
+                    q.get(timeout=0.1)
+                except queue.Empty:
+                    pass
+            worker.join()
+
+
+class ImageFolderImagenet:
+    """train_loader / test_loader pair over ``{dataset_params.data_root_dir}/{train,val}``, the shape of the
+    reference's ``FFCVImagenet`` (utils/dataset.py:347-430): batch ``total_batch_size // world_size``, ``num_workers``
+    reading threads, seeded by ``experiment_params.seed``."""
+
+    def __init__(self, cfg, device, world_size=1, rank=0):
+        dp = cfg.dataset_params
+        kw = dict(total_batch_size=dp.total_batch_size, device=device, num_workers=getattr(dp, "num_workers", 8),
+                  seed=cfg.experiment_params.seed, world_size=world_size, rank=rank)
+        self.train_loader = ImageFolderLoader(os.path.join(dp.data_root_dir, "train"), train=True, **kw)
+        self.test_loader = ImageFolderLoader(os.path.join(dp.data_root_dir, "val"), train=False, **kw)
