@@ -23,13 +23,9 @@ def run(n, nseg, density, kind=0, reps=7, flush=True):
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record(); plan.enqueue(k); b.record(); torch.cuda.synchronize()
         ts.append(a.elapsed_time(b))
-        # phase stamps of this call (CTA 0, %globaltimer): SelState sits behind the segment table in the workspace; read
-        # before finish() — its exact fallback (experiment builds that break the bracket) reuses the state
-        off = (nseg * 64 + 255) // 256 * 256                  # sizeof(Seg) = 64
-        raw = bytes(plan.wsb[off:off + 256].cpu().numpy().tobytes())
+        # phase stamps of this call (CTA 0, %globaltimer), read before finish(): its exact fallback reuses the state
+        tp = plan.state()["t_phase"]
         _, thr, info = plan.finish(k)
-    import struct
-    tp = struct.unpack_from("<8Q", raw, 8 * 4 + 4 * 4 + 4 * 2 + 4 * 2 + 8 * 4 + 8)   # after k,n_lt,n_eq,n_cand | lo,hi,thr,status | prefix,mask | c_lo,c_hi | before_lo,before_hi,k_rem,n_cand2 | barrier,pad
     names = ["P0 sample", "P1 refine", "P2 sweep", "P3 decide", "P4 narrow", "P5 finish"]
     ph = ", ".join(f"{n} {(tp[i + 1] - tp[i]) / 1e3:.1f}" for i, n in enumerate(names) if tp[i + 1] > tp[i] > 0)
     t = statistics.median(ts); bpe = 12 if kind == 0 else 16

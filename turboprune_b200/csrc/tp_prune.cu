@@ -4,7 +4,7 @@
 // (per-layer score temporaries, torch.cat, single-CTA 16-pass torch.kthvalue, per-layer
 // torch.where) with ONE kernel of resident CTAs (k_topk_fused) whose phases are separated by grid-wide barriers:
 //
-//   P0 sample   : 2^20 strided samples (runs of 4 neighbours), kept in shared memory; 2048-bin histogram of key
+//   P0 sample   : 2^20 strided samples (runs of 16 neighbours), kept in shared memory; 2048-bin histogram of key
 //                 bits [30:20], shared-memory privatised
 //   P1 refine   : every CTA locates the coarse bins of the two bracket ranks (sample quantile +- 5 sigma of its
 //                 rank error) and histograms bits [19:9] of its own samples inside them
@@ -197,8 +197,8 @@ __global__ void __launch_bounds__(kSweepThreads) k_topk_fused(const TopkArgs a) 
   unsigned int* hist_f = a.hist + kDigitBins;
   unsigned int* hist_r = a.hist + 3 * kDigitBins;
 
-  // ---------------- P0: strided sample in runs of 4 neighbouring elements (one 32-byte sector per operand serves 4
-  // samples), keys stay in shared memory; coarse histogram of key bits [30:20] ----------------
+  // ---------------- P0: strided sample in runs of kRun = 16 neighbouring elements (one 64-byte burst per operand serves
+  // 16 samples), keys stay in shared memory; coarse histogram of key bits [30:20] ----------------
   stamp(st, 0);
   GridBarrier grid; grid.ctr = &st->barrier; grid.target = 0;
   const bool seg_smem = a.n_seg <= kSmemSegs;

@@ -225,6 +225,35 @@ class TopKPlan:
         self.enqueue(k)
         return self.finish(k)
 
+    def state(self):
+        """The selection state the last ``enqueue`` left in the workspace (see ``topk_state``)."""
+        return topk_state(self.wsb, self.n)
+
+
+# SelState of tp_prune.cu: k, n_lt, n_eq, n_cand | lo, hi, thr_key, status | prefix, prefix_mask | c_lo, c_hi |
+# before_lo, before_hi, k_rem, n_cand2 | barrier, pad | t_phase[8]
+_SELSTATE = ("<QQQQ IIIi II II QQQQ II 8Q", ("k", "n_lt", "n_eq", "n_cand", "lo", "hi", "thr_key", "status", "prefix",
+                                           "prefix_mask", "c_lo", "c_hi", "before_lo", "before_hi", "k_rem", "n_cand2",
+                                           "barrier", "pad"))
+
+
+def topk_state(wsb, n_seg):
+    """Decode the top-k selection state from a workspace of ``tp_topk_*``: a dict of the SelState fields, ``t_phase``
+    (the %globaltimer stamps of CTA 0) and ``hist`` (uint32 [8192]: the coarse sample histogram, the two fine ones and
+    the candidates' top-digit histogram).  The state follows the segment table (64 B per segment) at a 256-byte
+    boundary, its histograms at the next one.  Read it after ``enqueue`` and before ``finish``: the exact fallback
+    that ``finish`` may run rewrites it."""
+    import struct
+    import numpy as np
+    off = (64 * n_seg + 255) // 256 * 256
+    raw = wsb[off:off + 256 + 4 * 4 * 2048].cpu().numpy().tobytes()
+    fmt, names = _SELSTATE
+    vals = struct.unpack_from(fmt.replace(" ", ""), raw, 0)
+    st = dict(zip(names, vals[:len(names)]))
+    st["t_phase"] = list(vals[len(names):])
+    st["hist"] = np.frombuffer(raw, dtype=np.uint32, offset=256).copy()
+    return st
+
 
 def apply_threshold(ws, ms, thr, gs=None, kind=_cabi.TP_SCORE_MAG):
     lib = _cabi.load()
