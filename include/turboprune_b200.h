@@ -34,7 +34,8 @@ extern "C" {
 
 const char* tp_strerror(int code);
 const char* tp_last_cuda_error(void);      /* text of the last CUDA error seen by this thread */
-int         tp_abi_version(void);          /* bumps when a signature changes; 9: tp_cifar_augment takes idx; 10: tp_resized_crop */
+int         tp_abi_version(void);          /* bumps when a signature changes; 9: tp_cifar_augment takes idx; 10: tp_resized_crop;
+                                              11: the fp32 (TF32) training entry points */
 int         tp_device_sm_count(void);      /* cached multiprocessor count of the current device */
 /* Programmatic dependent launch for the train-step kernels (default off; TP_PDL=1 in the environment turns it on).
  * Returns the previous setting.  A debugging / A-B switch: results are bit-identical either way. */
@@ -239,6 +240,39 @@ int tp_conv_dgrad_bnrelu(const tp_conv_desc* d, const void* dy, const void* wd, 
  * computed nor read back, their gradient is written as zero — the result is the dense walk's, bit for bit. */
 int tp_conv_wgrad(const tp_conv_desc* d, const void* x, const void* dy, const void* mask, const void* kmask_f,
                   int cin_real, void* dw, void* db, void* ws, size_t ws_bytes, void* stream);
+
+/* ---- fp32 training (experiment_params.training_precision: float32) ----------------------
+ * The reference's float32 mode keeps every tensor fp32 and runs convolutions / matmuls on TF32 tensor cores
+ * (torch.backends.*.allow_tf32 = True).  These entry points are the fp32 counterparts of the calls above; the operand
+ * layouts, channel padding and tp_conv_desc are the bf16 ones.
+ *
+ * tp_conv_fprop_f32 / tp_conv_dgrad_f32: x / dy, wf / wd and y / dx are fp32 (NHWC, layouts of tp_stage_weights_f32),
+ * accumulation fp32 on TF32 wgmma.  The tensor core reads each operand's upper 19 bits (truncation of the low 13
+ * mantissa bits); the stored operands themselves are exact.  fprop adds the optional fp32 bias.  No statistics,
+ * BatchNorm-gate or addend epilogue and no K-block skipping.  Channel counts as for the bf16 calls (cin % 8 == 0,
+ * % 64 for filters with more than one tap). */
+int tp_conv_fprop_f32(const tp_conv_desc* d, const void* x, const void* wf, const void* bias_f32, void* y, void* stream);
+int tp_conv_dgrad_f32(const tp_conv_desc* d, const void* dy, const void* wd, void* dx, void* stream);
+/* The fp32 weight gradient runs as ONE bf16 tp_conv_wgrad over 3n images: TF32 wgmma cannot read the MN-major operands
+ * the pixel contraction needs.  tp_wgrad_split3 writes an fp32 [n][c][h][w] tensor (element strides) as NHWC bf16
+ * [3n][h][w][c_pad] (channels >= c zero): image block lo_block holds lo = bf16(v - bf16(v)), the other two hi = bf16(v).
+ * With x stacked with lo_block = 1 and dy with lo_block = 2, the wgrad sums x_hi dy_hi + x_lo dy_hi + x_hi dy_lo: about
+ * 2^-16 relative error per product.  The bias gradient must not come from that call's colsum (it counts dy_hi twice). */
+int tp_wgrad_split3(const void* src, int64_t sn, int64_t sc, int64_t sh, int64_t sw,
+                    int n, int c, int h, int w, void* dst, int c_pad, int lo_block, void* stream);
+/* fp32 operand staging: the layouts of tp_stage_weights / tp_stage_weights_batched with fp32 elements, mask * w exact.
+ * No occupancy masks (items must have kmask_f = kmask_d = NULL).  wf / wd of the items point to fp32 buffers. */
+int tp_stage_weights_f32(const void* w, const void* mask, int cout, int cin, int r, int s,
+                         void* wf, int cin_p, int wf_ld, void* wd, int cout_p, void* stream);
+int tp_stage_weights_batched_f32(const tp_stage_item* items, int n_items, int table_cached, void* ws, size_t ws_bytes,
+                                 void* stream);
+/* fp32 [n][c][h][w] (element strides) -> NHWC fp32 [n][h][w][c_pad], channels >= c zero. */
+int tp_to_nhwc_f32(const void* src, int64_t sn, int64_t sc, int64_t sh, int64_t sw,
+                   int n, int c, int h, int w, void* dst, int c_pad, void* stream);
+/* tp_im2col_stem from an fp32 source to an fp32 matrix [n*p*q][kp] (kp % 8 == 0: 32-byte rows). */
+int tp_im2col_stem_f32(const void* src, int64_t sn, int64_t sc, int64_t sh, int64_t sw,
+                       int n, int c, int h, int w, int r, int s, int cg, int stride_h, int stride_w, int pad_h, int pad_w,
+                       int p, int q, void* xcol, int kp, void* stream);
 
 /* tp_bn_forward with the batch statistics supplied by the producing convolution (tp_conv_fprop_stats):
  * ext_stats [ext_rows][2][C] fp32 un-shifted sums; training must be non-zero.  ext_stats == NULL: identical to

@@ -90,6 +90,16 @@ SIGNATURES = {
     "tp_maxpool_backward": (c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 9 + [c_void_p]),
     "tp_p2p_allreduce_nvls": (c_int, [POINTER(c_void_p), POINTER(c_void_p), c_void_p, c_int, c_int, c_int64, c_void_p, c_float,
                                       c_void_p, c_int, c_void_p, c_void_p]),
+    # fp32 (TF32) training
+    "tp_conv_fprop_f32": (c_int, [POINTER(ConvDesc), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "tp_conv_dgrad_f32": (c_int, [POINTER(ConvDesc), c_void_p, c_void_p, c_void_p, c_void_p]),
+    "tp_wgrad_split3": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int,
+                                c_void_p]),
+    "tp_stage_weights_f32": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_int,
+                                     c_void_p]),
+    "tp_stage_weights_batched_f32": (c_int, [POINTER(StageItem), c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    "tp_to_nhwc_f32": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
+    "tp_im2col_stem_f32": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int64] + [c_int] * 13 + [c_void_p, c_int, c_void_p]),
 }
 
 

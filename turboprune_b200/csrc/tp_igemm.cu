@@ -201,7 +201,8 @@ __device__ __forceinline__ void decode_tile(const FwdParams& p, int tile, int n_
 
 // A K block of the fwd GEMM for one consumer warpgroup: D[128 x BLOCK_N] (+)= A[128 x 64] * B[BLOCK_N x 64]^T, both
 // K-major; rows 0..63 accumulate into acc[0 .. BLOCK_N/2), rows 64..127 into acc[BLOCK_N/2 .. BLOCK_N).
-template <int BLOCK_N>
+// T = float: the same block as 32 fp32 channels per 128-B row, four TF32 k8 MMAs per 64-row half.
+template <int BLOCK_N, typename T = __nv_bfloat16>
 __device__ __forceinline__ void fwd_mma_block(float (&acc)[BLOCK_N], uint32_t a_addr, uint32_t b_addr, uint32_t accumulate) {
   const uint64_t adesc = make_smem_desc(a_addr, 16, 1024);
   const uint64_t adesc_hi = make_smem_desc(a_addr + 64 * kBlockK * 2, 16, 1024);
@@ -209,7 +210,15 @@ __device__ __forceinline__ void fwd_mma_block(float (&acc)[BLOCK_N], uint32_t a_
 #pragma unroll
   for (int k = 0; k < kBlockK / 16; ++k) {
     // advance 16 elements (32 B) along K inside the 128-B swizzle row: +2 in 16-B units
-    if constexpr (BLOCK_N == 128) {
+    if constexpr (sizeof(T) == 4) {           // 8 tf32 elements: also 32 B
+      if constexpr (BLOCK_N == 128) {
+        wgmma_m64n128_tf32(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), accumulate | (uint32_t)k);
+        wgmma_m64n128_tf32(acc + BLOCK_N / 2, adesc_hi + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), accumulate | (uint32_t)k);
+      } else {
+        wgmma_m64n64_tf32(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), accumulate | (uint32_t)k);
+        wgmma_m64n64_tf32(acc + BLOCK_N / 2, adesc_hi + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), accumulate | (uint32_t)k);
+      }
+    } else if constexpr (BLOCK_N == 128) {
       wgmma_m64n128<0, 0>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), accumulate | (uint32_t)k);
       wgmma_m64n128<0, 0>(acc + BLOCK_N / 2, adesc_hi + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), accumulate | (uint32_t)k);
     } else {
@@ -239,12 +248,23 @@ __device__ __forceinline__ void fwd_mma_block(float (&acc)[BLOCK_N], uint32_t a_
 // and writes them into the warpgroup's 128 x 64 bf16 staging tile (16-byte chunk j of row r at chunk j ^ (r & 7):
 // conflict-free for the fragment stores and for the row reads); after a warpgroup barrier, warp q reads rows
 // 32q .. 32q+31 back row-coalesced for full-line stores, the BatchNorm statistics and the BNB gate.
-template <int BLOCK_N, bool MULTI, bool BNB>
+//
+// T = float (TF32 mode): activations, weights and the output are fp32 (p.out points to float).  The stage ring is the
+// same bytes: a 128-B swizzle row holds 32 fp32 instead of 64 bf16, so a K block is 32 channels and cchunks counts
+// 32-channel blocks.  Operands are read by TMA as plain FLOAT32 (not the TFLOAT32 map type, which may round), and the
+// tensor core truncates each to its upper 19 bits (tp_ptx.cuh).  No K-block skipping (dense walk).  The epilogue adds
+// the bias and stores each thread's fragments directly: a quad of lanes writes two adjacent fp32 of 4 consecutive column
+// pairs, i.e. one full 32-byte sector per row, so no staging tile is needed.  No statistics, BNB or addend epilogue:
+// the fp32 model runs BatchNorm, ReLU and the residual add as separate fp32 ops.
+template <int BLOCK_N, bool MULTI, bool BNB, typename T = __nv_bfloat16>
 __global__ void __launch_bounds__(kFwdThreads, 1)
 k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ FwdParams p) {
   static_assert(BLOCK_N == 64 || BLOCK_N == 128, "wgmma N of the fwd kernel");
   static_assert(!BNB || !MULTI, "BatchNorm-backward epilogue: single class");
+  constexpr bool kF32 = sizeof(T) == 4;
+  static_assert(!kF32 || !BNB, "fp32 operands: no BatchNorm-backward epilogue");
+  constexpr int kKe = 128 / (int)sizeof(T);                // channels of one K block: one 128-B swizzle row
   constexpr int kABytes = kBlockM * kBlockK * 2;           // 16 KB
   constexpr int kBBytes = BLOCK_N * kBlockK * 2;
   constexpr int kStageBytes = kABytes + kBBytes;
@@ -289,7 +309,7 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
     setmaxnreg_dec<kFwdProducerRegs>();
     if (threadIdx.x == 0) {
       int stage = 0; uint32_t phase = 0;
-      const uint32_t* const km = live_kmask(p.kmask, p.kmask_words, p.N);
+      const uint32_t* const km = kF32 ? nullptr : live_kmask(p.kmask, p.kmask_words, p.N);
       for (int w = 0; w < my_items; ++w) {
         int ci, m_g, n_t; get_tile(w, ci, m_g, n_t);
         const ClsEntry& ce = p.cls[MULTI ? ci : 0];
@@ -304,10 +324,10 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
           uint8_t* sB = sA + kABytes;
           mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
           if (p.a_mode == 1)
-            tma_load_im2col_4d(sA, mapA, &full_bar[stage], cc * kBlockK, cw, ch, cn, te.off_w, te.off_h);
+            tma_load_im2col_4d(sA, mapA, &full_bar[stage], cc * kKe, cw, ch, cn, te.off_w, te.off_h);
           else
-            tma_load_2d(sA, mapA, &full_bar[stage], te.kofs + cc * kBlockK, m0);
-          tma_load_2d(sB, &tmB, &full_bar[stage], te.kofs + cc * kBlockK, n_t * BLOCK_N);
+            tma_load_2d(sA, mapA, &full_bar[stage], te.kofs + cc * kKe, m0);
+          tma_load_2d(sB, &tmB, &full_bar[stage], te.kofs + cc * kKe, n_t * BLOCK_N);
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         };
         const int tap_base = MULTI ? ce.tap0 : 0;     // single class: a static table offset (no dependent parameter load)
@@ -340,7 +360,7 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
     const int q = warp & 3;                   // epilogue: rows 32q .. 32q+31 of the tile, one per lane
     const int wtid = threadIdx.x & 127;
     const int bar_id = 1 + cw;                // warpgroup-local named barrier
-    const uint32_t* const km = live_kmask(p.kmask, p.kmask_words, p.N);
+    const uint32_t* const km = kF32 ? nullptr : live_kmask(p.kmask, p.kmask_words, p.N);
     const uint32_t stg = smem_u32(stg_base + cw * kStgBytes);
     // fragment rows of this thread: fr0 + 8h + 64mh (h, mh in {0, 1}); their swizzle key (row & 7) is lane / 4
     const int fr0 = q * 16 + (lane >> 2);
@@ -381,7 +401,7 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
           mbar_wait(&full_bar[stage], phase);
           const uint32_t s_addr = smem_u32(smem + stage * kStageBytes);
           wgmma_fence();
-          fwd_mma_block<BLOCK_N>(acc, s_addr, s_addr + kABytes, accumulate);
+          fwd_mma_block<BLOCK_N, T>(acc, s_addr, s_addr + kABytes, accumulate);
           wgmma_commit();
           wgmma_wait<1>();
           if (prev >= 0 && wtid == 0) mbar_arrive(&empty_bar[prev]);
@@ -428,6 +448,41 @@ k_igemm_fwd(const __grid_constant__ AMaps tmA, const __grid_constant__ CUtensorM
         }
       }
       auto row_off = [&](int i) -> long long { return MULTI ? ooff[MULTI ? i : 0] : rbase + (long long)(i * 4) * ldc; };
+      if constexpr (kF32) {
+        // fp32 output: (+ bias) and direct stores of the fragments; a parity class no tap reaches is written as zeros
+        float* const out = reinterpret_cast<float*>(p.out);
+        const bool pair_ok = (p.ldc & 1) == 0 && (((uintptr_t)out) & 7) == 0;
+#pragma unroll
+        for (int mh = 0; mh < 2; ++mh)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = m_t * kBlockM + fr0 + 8 * h + 64 * mh;
+            if (row >= ce.M) continue;
+            long long opix = row;
+            if (MULTI || !p.linear) {
+              int n, pp, qq; decompose_pixel(row, ce.P_it, ce.Q_it, n, pp, qq);
+              opix = (long long)n * p.out_img_pix + (long long)(pp * p.osh + ce.oah) * p.out_row_pix + (qq * p.osw + ce.oaw);
+            }
+            float* const orow = out + opix * p.ldc;
+#pragma unroll
+            for (int j = 0; j < BLOCK_N / 8; ++j) {
+              const int n = n_t * BLOCK_N + 8 * j + 2 * (lane & 3);
+              if (n >= N) continue;
+              const int i = mh * (BLOCK_N / 2) + 4 * j + 2 * h;
+              float f0 = has_acc ? acc[i] : 0.f, f1 = has_acc ? acc[i + 1] : 0.f;
+              if (p.bias && has_acc) {
+                f0 += p.bias[n];
+                if (n + 1 < N) f1 += p.bias[n + 1];
+              }
+              if (n + 1 < N && pair_ok) *reinterpret_cast<float2*>(orow + n) = make_float2(f0, f1);
+              else {
+                orow[n] = f0;
+                if (n + 1 < N) orow[n + 1] = f1;
+              }
+            }
+          }
+        continue;
+      }
       if (MULTI && !has_acc) {
         // parity class no tap reaches (e.g. 3 of the 4 classes of a 1x1 stride-2 convolution): dX there is the fused addend
         // or zero — plain coalesced copies / stores
@@ -928,12 +983,16 @@ static int fail_cu(CUresult r, const char* what) {
 }
 
 // 2-D bf16 tensor [rows][cols] (cols contiguous, row stride ld elements), box = [box_rows][64 cols], SW128.
-static int make_tiled_map(CUtensorMap* m, const void* ptr, uint64_t cols, uint64_t rows, uint64_t ld_elems, uint32_t box_rows) {
+// f32: an fp32 tensor, box = [box_rows][32 cols] (the same 128-B rows).  FLOAT32, not TFLOAT32: the map type that rounds
+// to tf32 on load is not used, the tensor core's truncation is the only operand rounding.
+static int make_tiled_map(CUtensorMap* m, const void* ptr, uint64_t cols, uint64_t rows, uint64_t ld_elems, uint32_t box_rows,
+                          bool f32 = false) {
   cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld_elems * 2};
-  cuuint32_t box[2] = {64, box_rows};
+  cuuint64_t strides[1] = {ld_elems * (f32 ? 4 : 2)};
+  cuuint32_t box[2] = {f32 ? 32u : 64u, box_rows};
   cuuint32_t es[2] = {1, 1};
-  CUresult r = g_encodeTiled(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, es,
+  CUresult r = g_encodeTiled(m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr),
+                             dims, strides, box, es,
                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                              CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail_cu(r, "cuTensorMapEncodeTiled");
@@ -942,21 +1001,24 @@ static int make_tiled_map(CUtensorMap* m, const void* ptr, uint64_t cols, uint64
 
 // im2col map over NHWC bf16 [n][h][w][c]: `pixels` consecutive iteration positions x 64 channels.
 // Iteration grid (P_it x Q_it per image) starts at (base_h, base_w) and advances by (step_h, step_w).
+// f32: NHWC fp32, 32 channels per pixel row (128 B).
 static int make_im2col_map(CUtensorMap* m, const void* ptr, int n, int h, int w, int c,
-                           int base_w, int base_h, int step_w, int step_h, int P_it, int Q_it, uint32_t pixels) {
+                           int base_w, int base_h, int step_w, int step_h, int P_it, int Q_it, uint32_t pixels, bool f32 = false) {
+  const cuuint64_t es_b = f32 ? 4 : 2;
   cuuint64_t dims[4] = {(cuuint64_t)c, (cuuint64_t)w, (cuuint64_t)h, (cuuint64_t)n};
-  cuuint64_t strides[3] = {(cuuint64_t)c * 2, (cuuint64_t)w * c * 2, (cuuint64_t)h * w * c * 2};
+  cuuint64_t strides[3] = {(cuuint64_t)c * es_b, (cuuint64_t)w * c * es_b, (cuuint64_t)h * w * c * es_b};
   // bounding box: base positions run from `lower` while < extent + upper  =>  count = Q_it
   int lower[2] = {base_w, base_h};
   int upper[2] = {(Q_it - 1) * step_w + 1 + base_w - w, (P_it - 1) * step_h + 1 + base_h - h};
   cuuint32_t es[4] = {1, (cuuint32_t)step_w, (cuuint32_t)step_h, 1};
-  CUresult r = g_encodeIm2col(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr), dims, strides, lower, upper,
-                              64, pixels, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+  CUresult r = g_encodeIm2col(m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(ptr),
+                              dims, strides, lower, upper,
+                              f32 ? 32 : 64, pixels, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                               CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail_cu(r, "cuTensorMapEncodeIm2col");
   // Driver quirk (CUDA <= 13.1 drivers, see CUTLASS copy_traits_sm90_im2col.hpp): for tensors
   // smaller than 128 KiB bit 21 of the second descriptor word must be cleared.
-  if (g_driver_version <= 13010 && (size_t)n * h * w * c * 2 < 131072)
+  if (g_driver_version <= 13010 && (size_t)n * h * w * c * es_b < 131072)
     reinterpret_cast<uint64_t*>(m)[1] &= ~(1ull << 21);
   return TP_OK;
 }
@@ -1043,14 +1105,14 @@ static int pick_block_n(long long m_tiles, int n) {
 
 constexpr int kSmemMax = 232448;                 // 227 KB: the per-CTA opt-in limit of sm_90
 
-template <int BN, bool MULTI, bool BNB = false>
+template <int BN, bool MULTI, bool BNB = false, typename T = __nv_bfloat16>
 static int launch_fwd(const AMaps& a, const CUtensorMap& b, FwdParams& p, cudaStream_t st) {
   constexpr int smem = fwd_smem(BN);
   static_assert(smem <= kSmemMax, "fwd smem budget");
   const int n_tiles = (p.N + BN - 1) / BN;
   static bool attr_set = false;
   if (!attr_set) {
-    TP_CUDA_CHECK(cudaFuncSetAttribute(k_igemm_fwd<BN, MULTI, BNB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    TP_CUDA_CHECK(cudaFuncSetAttribute(k_igemm_fwd<BN, MULTI, BNB, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_set = true;
   }
   // work items: per class, (M tiles) x (N tiles), classes back to back
@@ -1063,16 +1125,27 @@ static int launch_fwd(const AMaps& a, const CUtensorMap& b, FwdParams& p, cudaSt
   }
   if (ctiles > 0x7fffffffll || ctiles <= 0) return TP_ERR_UNSUPPORTED;
   const int grid = (int)(ctiles < sm_count() ? ctiles : sm_count());
-  TP_CUDA_CHECK(launch(k_igemm_fwd<BN, MULTI, BNB>, dim3(grid), dim3(kFwdThreads), (size_t)smem, st, a, b, p));
+  TP_CUDA_CHECK(launch(k_igemm_fwd<BN, MULTI, BNB, T>, dim3(grid), dim3(kFwdThreads), (size_t)smem, st, a, b, p));
   TP_LAUNCH_CHECK();
   return TP_OK;
 }
 
-static int run_fwd(const AMaps& a, const CUtensorMap& b, FwdParams& p, int bn, cudaStream_t st) {
+static int run_fwd(const AMaps& a, const CUtensorMap& b, FwdParams& p, int bn, cudaStream_t st, bool f32 = false) {
   // 16-byte aligned output rows -> the epilogue stages 32x64 sub-tiles through smem and writes full 128-byte lines
   // (for any pixel mapping: a strided dgrad's parity classes compute the destination pixel of each row)
   p.linear = p.ncls == 1 && p.osh == 1 && p.osw == 1 && p.cls[0].oah == 0 && p.cls[0].oaw == 0 &&
              p.out_row_pix == p.cls[0].Q_it && p.out_img_pix == (long long)p.cls[0].P_it * p.cls[0].Q_it;
+  if (f32) {
+    // fp32 operands and output: bias only (no statistics, BatchNorm gate or addend), fragments stored directly
+    if (p.stats || p.bn_y || p.addend || p.kmask) return TP_ERR_UNSUPPORTED;
+    p.staged_store = 0;
+    if (!p.linear) {
+      if (bn == 128) return launch_fwd<128, true, false, float>(a, b, p, st);
+      return launch_fwd<64, true, false, float>(a, b, p, st);
+    }
+    if (bn == 128) return launch_fwd<128, false, false, float>(a, b, p, st);
+    return launch_fwd<64, false, false, float>(a, b, p, st);
+  }
   p.staged_store = (p.ldc % 8 == 0 && p.N % 8 == 0 && (((uintptr_t)p.out) & 15) == 0 &&
                     (!p.addend || (((uintptr_t)p.addend) & 15) == 0)) ? 1 : 0;
   if (p.stats && !(p.staged_store && p.linear)) return TP_ERR_UNSUPPORTED;
@@ -1130,9 +1203,21 @@ int tp_conv_fprop(const tp_conv_desc* d, const void* x, const void* wf, const vo
   return tp_conv_fprop_stats(d, x, wf, nullptr, bias_f32, y, nullptr, ws, ws_bytes, stream);
 }
 
+static int conv_fprop_impl(const tp_conv_desc* d, const void* x, const void* wf, const void* kmask_f, const void* bias_f32,
+                           void* y, void* stats, void* stream, bool f32);
+
 int tp_conv_fprop_stats(const tp_conv_desc* d, const void* x, const void* wf, const void* kmask_f, const void* bias_f32,
                         void* y, void* stats, void* ws, size_t ws_bytes, void* stream) {
   (void)ws; (void)ws_bytes;
+  return conv_fprop_impl(d, x, wf, kmask_f, bias_f32, y, stats, stream, false);
+}
+
+int tp_conv_fprop_f32(const tp_conv_desc* d, const void* x, const void* wf, const void* bias_f32, void* y, void* stream) {
+  return conv_fprop_impl(d, x, wf, nullptr, bias_f32, y, nullptr, stream, true);
+}
+
+static int conv_fprop_impl(const tp_conv_desc* d, const void* x, const void* wf, const void* kmask_f, const void* bias_f32,
+                           void* y, void* stats, void* stream, bool f32) {
   if (!d || !x || !wf || !y) return TP_ERR_INVALID;
   if (stats && (d->cout % 8 != 0 || (((uintptr_t)y) & 15) != 0 || (((uintptr_t)stats) & 15) != 0)) return TP_ERR_UNSUPPORTED;
   if (d->cin % 8 != 0 || d->r * d->s > kMaxTaps) return TP_ERR_UNSUPPORTED;
@@ -1145,7 +1230,8 @@ int tp_conv_fprop_stats(const tp_conv_desc* d, const void* x, const void* wf, co
   p.ncls = 1;
   ClsEntry& ce = p.cls[0];
   ce.M = p.M; ce.P_it = d->p; ce.Q_it = d->q; ce.ntaps = d->r * d->s; ce.tap0 = 0; ce.oah = 0; ce.oaw = 0;
-  p.cchunks = (d->cin + 63) / 64;
+  const int ke = f32 ? 32 : 64;                  // channels per K block
+  p.cchunks = (d->cin + ke - 1) / ke;
   p.out_img_pix = (long long)d->p * d->q; p.out_row_pix = d->q;
   p.osh = 1; p.osw = 1;
   p.ldc = d->cout; p.out = (__nv_bfloat16*)y; p.bias = (const float*)bias_f32;
@@ -1155,29 +1241,33 @@ int tp_conv_fprop_stats(const tp_conv_desc* d, const void* x, const void* wf, co
   AMaps ta; CUtensorMap tb;
   if (is_plain_gemm(d)) {
     p.a_mode = 0;
-    rc = make_tiled_map(&ta.m[0], x, (uint64_t)d->cin, (uint64_t)p.M, (uint64_t)d->cin, kBlockM); if (rc) return rc;
+    rc = make_tiled_map(&ta.m[0], x, (uint64_t)d->cin, (uint64_t)p.M, (uint64_t)d->cin, kBlockM, f32); if (rc) return rc;
   } else {
     p.a_mode = 1;
     ce.base_w = -d->pad_w; ce.base_h = -d->pad_h; p.step_w = d->stride_w; p.step_h = d->stride_h;
-    rc = make_im2col_map(&ta.m[0], x, d->n, d->h, d->w, d->cin, ce.base_w, ce.base_h, p.step_w, p.step_h, d->p, d->q, kBlockM);
+    rc = make_im2col_map(&ta.m[0], x, d->n, d->h, d->w, d->cin, ce.base_w, ce.base_h, p.step_w, p.step_h, d->p, d->q, kBlockM, f32);
     if (rc) return rc;
   }
   for (int c = 1; c < kMaxCls; ++c) ta.m[c] = ta.m[0];
   const int bn = pick_block_n((p.M + kBlockM - 1) / kBlockM, p.N);
-  rc = make_tiled_map(&tb, wf, (uint64_t)d->r * d->s * d->cin, (uint64_t)d->cout, (uint64_t)d->r * d->s * d->cin, (uint32_t)bn);
+  rc = make_tiled_map(&tb, wf, (uint64_t)d->r * d->s * d->cin, (uint64_t)d->cout, (uint64_t)d->r * d->s * d->cin, (uint32_t)bn, f32);
   if (rc) return rc;
-  return run_fwd(ta, tb, p, bn, st);
+  return run_fwd(ta, tb, p, bn, st, f32);
 }
 
 struct BnGate { const void* y; const float* weight; const float* bias; const float* mean; const float* invstd; float* partial; };
 
 static int conv_dgrad_impl(const tp_conv_desc* d, const void* dy, const void* wd, const void* kmask_d, const void* addend,
-                           void* dx, const BnGate* gate, void* stream);
+                           void* dx, const BnGate* gate, void* stream, bool f32 = false);
 
 int tp_conv_dgrad(const tp_conv_desc* d, const void* dy, const void* wd, const void* kmask_d, const void* addend,
                   void* dx, void* ws, size_t ws_bytes, void* stream) {
   (void)ws; (void)ws_bytes;
   return conv_dgrad_impl(d, dy, wd, kmask_d, addend, dx, nullptr, stream);
+}
+
+int tp_conv_dgrad_f32(const tp_conv_desc* d, const void* dy, const void* wd, void* dx, void* stream) {
+  return conv_dgrad_impl(d, dy, wd, nullptr, nullptr, dx, nullptr, stream, true);
 }
 
 int tp_conv_dgrad_bnrelu(const tp_conv_desc* d, const void* dy, const void* wd, const void* kmask_d,
@@ -1198,7 +1288,7 @@ size_t tp_conv_dgrad_partial_rows(const tp_conv_desc* d) {
 }
 
 static int conv_dgrad_impl(const tp_conv_desc* d, const void* dy, const void* wd, const void* kmask_d, const void* addend,
-                           void* dx, const BnGate* gate, void* stream) {
+                           void* dx, const BnGate* gate, void* stream, bool f32) {
   if (!d || !dy || !wd || !dx) return TP_ERR_INVALID;
   // here the contraction runs over (r', s', cout): channel count of dY must be TMA friendly
   const int cop = d->cout;                       // caller passes dY with cout % 8 == 0 (padded if needed)
@@ -1212,7 +1302,7 @@ static int conv_dgrad_impl(const tp_conv_desc* d, const void* dy, const void* wd
   const int sh = d->stride_h, sw = d->stride_w;
   FwdParams p = {};
   p.N = d->cin;
-  p.cchunks = (cop + 63) / 64;
+  p.cchunks = f32 ? (cop + 31) / 32 : (cop + 63) / 64;
   p.out_img_pix = (long long)d->h * d->w; p.out_row_pix = d->w;
   p.ldc = d->cin; p.out = (__nv_bfloat16*)dx; p.bias = nullptr; p.addend = (const __nv_bfloat16*)addend;
   p.kmask = (const uint32_t*)kmask_d; p.kmask_words = (int)tp_kblock_mask_words(ktot);
@@ -1231,11 +1321,11 @@ static int conv_dgrad_impl(const tp_conv_desc* d, const void* dy, const void* wd
     fill_taps(p.taps, R, S, cop);
     if (is_plain_gemm(d)) {
       p.a_mode = 0;
-      rc = make_tiled_map(&ta.m[0], dy, (uint64_t)cop, (uint64_t)p.M, (uint64_t)cop, kBlockM); if (rc) return rc;
+      rc = make_tiled_map(&ta.m[0], dy, (uint64_t)cop, (uint64_t)p.M, (uint64_t)cop, kBlockM, f32); if (rc) return rc;
     } else {
       p.a_mode = 1;
       ce.base_w = -(S - 1 - d->pad_w); ce.base_h = -(R - 1 - d->pad_h);
-      rc = make_im2col_map(&ta.m[0], dy, d->n, d->p, d->q, cop, ce.base_w, ce.base_h, 1, 1, d->h, d->w, kBlockM);
+      rc = make_im2col_map(&ta.m[0], dy, d->n, d->p, d->q, cop, ce.base_w, ce.base_h, 1, 1, d->h, d->w, kBlockM, f32);
       if (rc) return rc;
     }
     for (int c = 1; c < kMaxCls; ++c) ta.m[c] = ta.m[0];
@@ -1270,7 +1360,7 @@ static int conv_dgrad_impl(const tp_conv_desc* d, const void* dy, const void* wd
         }
       } else { dh_min = 0; dw_min = 0; }
       ce.base_w = dw_min; ce.base_h = dh_min;
-      rc = make_im2col_map(&ta.m[nc], dy, d->n, d->p, d->q, cop, ce.base_w, ce.base_h, 1, 1, Hc, Wc, kBlockM); if (rc) return rc;
+      rc = make_im2col_map(&ta.m[nc], dy, d->n, d->p, d->q, cop, ce.base_w, ce.base_h, 1, 1, Hc, Wc, kBlockM, f32); if (rc) return rc;
       Mtot += ce.M; ++nc;
     }
     if (nc == 0) return TP_OK;
@@ -1280,8 +1370,8 @@ static int conv_dgrad_impl(const tp_conv_desc* d, const void* dy, const void* wd
   long long m_tiles = 0;
   for (int c = 0; c < p.ncls; ++c) m_tiles += (p.cls[c].M + kBlockM - 1) / kBlockM;
   const int bn = pick_block_n(m_tiles, p.N);
-  rc = make_tiled_map(&tb, wd, (uint64_t)ktot, (uint64_t)d->cin, (uint64_t)ktot, (uint32_t)bn); if (rc) return rc;
-  return run_fwd(ta, tb, p, bn, st);
+  rc = make_tiled_map(&tb, wd, (uint64_t)ktot, (uint64_t)d->cin, (uint64_t)ktot, (uint32_t)bn, f32); if (rc) return rc;
+  return run_fwd(ta, tb, p, bn, st, f32);
 }
 
 int tp_conv_wgrad(const tp_conv_desc* d, const void* x, const void* dy, const void* mask, const void* kmask_f,

@@ -21,9 +21,16 @@ constexpr int kSlabFloats = 8192;            // 32 KB
 // columns), set when the block holds a non-zero masked weight.  kmf: rows = output channels, column = tap*cin_p + ci (wf);
 // kmd: rows = input channels, column = rot_tap*cout_p + co (wd).  Bits are OR-ed into a buffer the host zeroed, so the
 // result does not depend on CTA order.
+//
+// T = float: the fp32 operands of the TF32 GEMMs, same layouts, mask * w stored exactly (no occupancy masks are asked for).
+template <typename T> __device__ __forceinline__ T to_operand(float v);
+template <> __device__ __forceinline__ __nv_bfloat16 to_operand<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+template <> __device__ __forceinline__ float to_operand<float>(float v) { return v; }
+
+template <typename T>
 __device__ __forceinline__ void stage_slab(const float* __restrict__ w, const float* __restrict__ mask, int co0, int cout,
-                                           int c0, int c1, int cin, int rs, __nv_bfloat16* __restrict__ wf, int cin_p, int wf_ld,
-                                           __nv_bfloat16* __restrict__ wd, int cout_p, bool zero_pad, float* s_slab,
+                                           int c0, int c1, int cin, int rs, T* __restrict__ wf, int cin_p, int wf_ld,
+                                           T* __restrict__ wd, int cout_p, bool zero_pad, float* s_slab,
                                            uint32_t* __restrict__ kmf, int kmf_words, uint32_t* __restrict__ kmd, int kmd_words) {
   const int t = threadIdx.x;
   const int cw = c1 - c0;                    // channels in this slice
@@ -46,7 +53,7 @@ __device__ __forceinline__ void stage_slab(const float* __restrict__ w, const fl
   for (int i = t; i < nco * per_co; i += blockDim.x) {
     const int cl = i / per_co, j = i - cl * per_co;
     const int tap = j / cw, c = j - tap * cw;
-    wf[(long long)(co0 + cl) * wf_ld + tap * cin_p + c0 + c] = __float2bfloat16_rn(s_slab[cl * per_co + c * rs + tap]);
+    wf[(long long)(co0 + cl) * wf_ld + tap * cin_p + c0 + c] = to_operand<T>(s_slab[cl * per_co + c * rs + tap]);
   }
   if (wd) {
     // wd[ci][rs-1-tap][co0 .. co0+8): one 16-byte store per (ci, tap); channels past cout are the zero padding
@@ -55,15 +62,20 @@ __device__ __forceinline__ void stage_slab(const float* __restrict__ w, const fl
       float f[kCoT];
 #pragma unroll
       for (int cl = 0; cl < kCoT; ++cl) f[cl] = cl < nco ? s_slab[cl * per_co + j] : 0.f;
-      __nv_bfloat16* dst = wd + ((long long)(c0 + c) * rs + (rs - 1 - tap)) * cout_p + co0;
+      T* dst = wd + ((long long)(c0 + c) * rs + (rs - 1 - tap)) * cout_p + co0;
       if (co0 + kCoT <= cout_p) {
-        uint4 v;
-        __nv_bfloat162* hv = reinterpret_cast<__nv_bfloat162*>(&v);
+        if constexpr (sizeof(T) == 4) {
+          reinterpret_cast<float4*>(dst)[0] = make_float4(f[0], f[1], f[2], f[3]);
+          reinterpret_cast<float4*>(dst)[1] = make_float4(f[4], f[5], f[6], f[7]);
+        } else {
+          uint4 v;
+          __nv_bfloat162* hv = reinterpret_cast<__nv_bfloat162*>(&v);
 #pragma unroll
-        for (int q = 0; q < 4; ++q) hv[q] = __floats2bfloat162_rn(f[2 * q], f[2 * q + 1]);
-        *reinterpret_cast<uint4*>(dst) = v;
+          for (int q = 0; q < 4; ++q) hv[q] = __floats2bfloat162_rn(f[2 * q], f[2 * q + 1]);
+          *reinterpret_cast<uint4*>(dst) = v;
+        }
       } else {
-        for (int cl = 0; cl < kCoT && co0 + cl < cout_p; ++cl) dst[cl] = __float2bfloat16_rn(f[cl]);
+        for (int cl = 0; cl < kCoT && co0 + cl < cout_p; ++cl) dst[cl] = to_operand<T>(f[cl]);
       }
     }
   }
@@ -105,15 +117,16 @@ __device__ __forceinline__ void stage_slab(const float* __restrict__ w, const fl
     for (int i = t; i < nco * padw * rs; i += blockDim.x) {
       const int cl = i / (padw * rs), j = i - cl * (padw * rs);
       const int tap = j / padw, c = j - tap * padw;
-      wf[(long long)(co0 + cl) * wf_ld + tap * cin_p + cin + c] = __float2bfloat16_rn(0.f);
+      wf[(long long)(co0 + cl) * wf_ld + tap * cin_p + cin + c] = to_operand<T>(0.f);
     }
   }
 }
 
+template <typename T>
 __global__ void __launch_bounds__(256) k_stage_weights(const float* __restrict__ w, const float* __restrict__ mask,
                                                        int cout, int cin, int rs,
-                                                       __nv_bfloat16* __restrict__ wf, int cin_p,
-                                                       __nv_bfloat16* __restrict__ wd, int cout_p, int wf_ld,
+                                                       T* __restrict__ wf, int cin_p,
+                                                       T* __restrict__ wd, int cout_p, int wf_ld,
                                                        uint32_t* __restrict__ kmf, int kmf_words,
                                                        uint32_t* __restrict__ kmd, int kmd_words) {
   pdl_enter();
@@ -136,6 +149,8 @@ struct StageItem {
   int kmf_words, kmd_words;
 };
 
+// T = float: wf / wd of the items point to fp32 buffers
+template <typename T>
 __global__ void __launch_bounds__(256) k_stage_weights_batched(const StageItem* __restrict__ items, int n_items) {
   pdl_enter();
   extern __shared__ float s_slab[];
@@ -150,8 +165,8 @@ __global__ void __launch_bounds__(256) k_stage_weights_batched(const StageItem* 
   const int ct = local / it.ysplit, y = local - ct * it.ysplit;
   const int c0 = y * it.cc, c1 = min(it.cin, c0 + it.cc);
   if (ct * kCoT >= it.cout || c0 >= c1) return;
-  stage_slab(it.w, it.mask, ct * kCoT, it.cout, c0, c1, it.cin, it.rs, it.wf, it.cin_p, it.wf_ld, it.wd, it.cout_p, false, s_slab,
-             it.kmf, it.kmf_words, it.kmd, it.kmd_words);
+  stage_slab(it.w, it.mask, ct * kCoT, it.cout, c0, c1, it.cin, it.rs, reinterpret_cast<T*>(it.wf), it.cin_p, it.wf_ld,
+             reinterpret_cast<T*>(it.wd), it.cout_p, false, s_slab, it.kmf, it.kmf_words, it.kmd, it.kmd_words);
 }
 
 // Number of EMPTY blocks of an occupancy mask, stored behind its last row: the GEMM kernels read this one word per CTA
@@ -213,6 +228,48 @@ __global__ void __launch_bounds__(256) k_to_nhwc(const T* __restrict__ src, long
     float v = 0.f;
     if (ci < c) v = (float)src[ni * sn + ci * sc + hi * sh + wi * sw];
     dst[i] = __float2bfloat16_rn(v);
+  }
+}
+
+// src[n][c][h][w] fp32 (any element strides) -> dst NHWC fp32 [n][h][w][c_pad], channels >= c zero (values unchanged)
+__global__ void __launch_bounds__(256) k_to_nhwc_f32(const float* __restrict__ src, long long sn, long long sc, long long sh, long long sw,
+                                                     int n, int c, int h, int w, float* __restrict__ dst, int c_pad) {
+  pdl_enter();
+  const long long total = (long long)n * h * w * c_pad;
+  long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (; i < total; i += stride) {
+    const int ci = (int)(i % c_pad);
+    const long long pix = i / c_pad;
+    const int wi = (int)(pix % w);
+    const long long t2 = pix / w;
+    const int hi = (int)(t2 % h), ni = (int)(t2 / h);
+    dst[i] = ci < c ? src[ni * sn + ci * sc + hi * sh + wi * sw] : 0.f;
+  }
+}
+
+// Three-way bf16 split of an fp32 operand for the fp32 weight gradient: dst NHWC bf16 [3n][h][w][c_pad] holds image
+// blocks b = 0, 1, 2 of n images each; block `lo_block` holds lo = bf16(v - hi), the other two hi = bf16(v).  v - hi is
+// exact in fp32, so hi + lo carries 16 significant bits of v.  Stacking x as (hi, lo, hi) and dy as (hi, hi, lo), ONE
+// bf16 wgrad over 3n images sums x_hi dy_hi + x_lo dy_hi + x_hi dy_lo.
+__global__ void __launch_bounds__(256) k_wgrad_split3(const float* __restrict__ src, long long sn, long long sc, long long sh, long long sw,
+                                                      int n, int c, int h, int w, __nv_bfloat16* __restrict__ dst, int c_pad,
+                                                      int lo_block) {
+  pdl_enter();
+  const long long total = (long long)n * h * w * c_pad;
+  long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (; i < total; i += stride) {
+    const int ci = (int)(i % c_pad);
+    const long long pix = i / c_pad;
+    const int wi = (int)(pix % w);
+    const long long t2 = pix / w;
+    const int hi_ = (int)(t2 % h), ni = (int)(t2 / h);
+    const float v = ci < c ? src[ni * sn + ci * sc + hi_ * sh + wi * sw] : 0.f;
+    const __nv_bfloat16 vh = __float2bfloat16_rn(v);
+    const __nv_bfloat16 vl = __float2bfloat16_rn(v - __bfloat162float(vh));
+#pragma unroll
+    for (int b = 0; b < 3; ++b) dst[i + b * total] = b == lo_block ? vl : vh;
   }
 }
 
@@ -294,12 +351,15 @@ __global__ void __launch_bounds__(256) k_im2col_stem(const T* __restrict__ src, 
 // of 8 halfwords from shared memory with loop-invariant offsets (thread = one cell column, walking the strip's pixels).
 // The per-cell kernel above spends its time on 8 bounds-checked scalar global loads + 8 table lookups + 3 divisions per
 // cell; this one has none of them in the inner loop.
-template <typename T>
+// TO = float: the fp32 matrix of the TF32 stem GEMM (the patch is staged as fp32, a cell is two 16-byte stores).
+template <typename T, typename TO = __nv_bfloat16>
 __global__ void __launch_bounds__(256) k_im2col_stem_rows(const T* __restrict__ src, long long sn, long long sc, long long sh, long long sw,
                                                           int n, int c, int h, int w, int R, int S, int cg, int stride_h, int stride_w,
                                                           int pad_h, int pad_w, int P, int Q, int QS, uint4* __restrict__ xcol, int kp8) {
   pdl_enter();
+  constexpr bool kF32 = sizeof(TO) == 4;
   extern __shared__ __align__(16) unsigned short s_patch[];      // [R][pw * c] bf16 bits, then one zero slot
+  float* const s_patch_f = reinterpret_cast<float*>(s_patch);    // TO = float: the same as fp32 values
   const int pw = (QS - 1) * stride_w + S;                       // input columns under a strip
   const int pitch = pw * c;
   const int zero_slot = R * pitch;
@@ -333,22 +393,33 @@ __global__ void __launch_bounds__(256) k_im2col_stem_rows(const T* __restrict__ 
         const int ww = w0 + wi;
         float v = 0.f;
         if (row_in && ww >= 0 && ww < w) v = (float)rowp[ww * sw + (long long)ch * sc];
-        s_patch[r * pitch + rem] = __bfloat16_as_ushort(__float2bfloat16_rn(v));
+        if constexpr (kF32) s_patch_f[r * pitch + rem] = v;
+        else s_patch[r * pitch + rem] = __bfloat16_as_ushort(__float2bfloat16_rn(v));
       }
     }
-    if (threadIdx.x == 0) s_patch[zero_slot] = 0;
+    if constexpr (kF32) { if (threadIdx.x == 0) s_patch_f[zero_slot] = 0.f; }
+    else { if (threadIdx.x == 0) s_patch[zero_slot] = 0; }
     __syncthreads();
     if (worker) {
       const long long row0 = ((long long)ni * P + pp) * Q + q0;
       for (int ql = plane; ql < nq; ql += cells_per_pass) {
         const int qo = ql * stride_w * c;
-        unsigned short hv[8];
+        if constexpr (kF32) {
+          float hf[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) hv[j] = s_patch[off[j] == zero_slot ? zero_slot : off[j] + qo];
-        uint4 v;
-        v.x = hv[0] | ((unsigned)hv[1] << 16); v.y = hv[2] | ((unsigned)hv[3] << 16);
-        v.z = hv[4] | ((unsigned)hv[5] << 16); v.w = hv[6] | ((unsigned)hv[7] << 16);
-        xcol[(row0 + ql) * kp8 + cell] = v;
+          for (int j = 0; j < 8; ++j) hf[j] = s_patch_f[off[j] == zero_slot ? zero_slot : off[j] + qo];
+          float4* const dst = reinterpret_cast<float4*>(xcol) + ((row0 + ql) * kp8 + cell) * 2;
+          dst[0] = make_float4(hf[0], hf[1], hf[2], hf[3]);
+          dst[1] = make_float4(hf[4], hf[5], hf[6], hf[7]);
+        } else {
+          unsigned short hv[8];
+#pragma unroll
+          for (int j = 0; j < 8; ++j) hv[j] = s_patch[off[j] == zero_slot ? zero_slot : off[j] + qo];
+          uint4 v;
+          v.x = hv[0] | ((unsigned)hv[1] << 16); v.y = hv[2] | ((unsigned)hv[3] << 16);
+          v.z = hv[4] | ((unsigned)hv[5] << 16); v.w = hv[6] | ((unsigned)hv[7] << 16);
+          xcol[(row0 + ql) * kp8 + cell] = v;
+        }
       }
     }
   }
@@ -434,7 +505,7 @@ int tp_stage_weights(const void* w, const void* mask, int cout, int cin, int r, 
   if (kmask_f) TP_CUDA_CHECK(cudaMemsetAsync(kmask_f, 0, ((size_t)((cout + 63) / 64) * kmf_words + 1) * 4, st));
   if (kmask_d && wd) TP_CUDA_CHECK(cudaMemsetAsync(kmask_d, 0, ((size_t)((cin + 63) / 64) * kmd_words + 1) * 4, st));
   dim3 grid((cout + kCoT - 1) / kCoT, ysplit);
-  launch(k_stage_weights, grid, 256, smem, st, (const float*)w, (const float*)mask, cout, cin, rs,
+  launch(k_stage_weights<__nv_bfloat16>, grid, 256, smem, st, (const float*)w, (const float*)mask, cout, cin, rs,
                                            (__nv_bfloat16*)wf, cin_p, (__nv_bfloat16*)wd, cout_p, wf_ld,
                                            (uint32_t*)kmask_f, kmf_words, (uint32_t*)kmask_d, kmd_words);
   if (kmask_f || (kmask_d && wd))
@@ -444,12 +515,45 @@ int tp_stage_weights(const void* w, const void* mask, int cout, int cin, int r, 
   return TP_OK;
 }
 
+int tp_stage_weights_f32(const void* w, const void* mask, int cout, int cin, int r, int s,
+                         void* wf, int cin_p, int wf_ld, void* wd, int cout_p, void* stream) {
+  if (!w || !mask || !wf || cout <= 0 || cin <= 0 || r <= 0 || s <= 0 || cin_p < cin) return TP_ERR_INVALID;
+  if (wd && cout_p < cout) return TP_ERR_INVALID;
+  if (wf_ld <= 0) wf_ld = r * s * cin_p;
+  if (wf_ld < r * s * cin_p) return TP_ERR_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int rs = r * s;
+  int max_c = kSlabFloats / (kCoT * rs); if (max_c < 1) return TP_ERR_UNSUPPORTED;
+  const int ysplit = (cin + max_c - 1) / max_c;
+  const int cc = (cin + ysplit - 1) / ysplit;
+  const size_t smem = (size_t)kCoT * cc * rs * sizeof(float);
+  if (wd && cout_p > cout) TP_CUDA_CHECK(cudaMemsetAsync(wd, 0, (size_t)cin * rs * cout_p * sizeof(float), st));
+  launch(k_stage_weights<float>, dim3((cout + kCoT - 1) / kCoT, ysplit), 256, smem, st, (const float*)w, (const float*)mask,
+         cout, cin, rs, (float*)wf, cin_p, (float*)wd, cout_p, wf_ld, (uint32_t*)nullptr, 0, (uint32_t*)nullptr, 0);
+  TP_LAUNCH_CHECK();
+  return TP_OK;
+}
+
 size_t tp_stage_batched_workspace_bytes(int n_items) {
   return n_items > 0 ? (size_t)n_items * sizeof(StageItem) + 512 : 0;
 }
 
+static int stage_batched_impl(const tp_stage_item* items, int n_items, int table_cached, void* kmask_all, size_t kmask_bytes,
+                              void* ws, size_t ws_bytes, void* stream, bool f32);
+
 int tp_stage_weights_batched(const tp_stage_item* items, int n_items, int table_cached, void* kmask_all, size_t kmask_bytes,
                              void* ws, size_t ws_bytes, void* stream) {
+  return stage_batched_impl(items, n_items, table_cached, kmask_all, kmask_bytes, ws, ws_bytes, stream, false);
+}
+
+int tp_stage_weights_batched_f32(const tp_stage_item* items, int n_items, int table_cached, void* ws, size_t ws_bytes, void* stream) {
+  for (int i = 0; items && i < n_items; ++i)
+    if (items[i].kmask_f || items[i].kmask_d) return TP_ERR_INVALID;          // fp32 operands carry no occupancy masks
+  return stage_batched_impl(items, n_items, table_cached, nullptr, 0, ws, ws_bytes, stream, true);
+}
+
+static int stage_batched_impl(const tp_stage_item* items, int n_items, int table_cached, void* kmask_all, size_t kmask_bytes,
+                              void* ws, size_t ws_bytes, void* stream, bool f32) {
   if (!items || n_items <= 0 || !ws) return TP_ERR_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
   Arena ar(ws, ws_bytes);
@@ -481,7 +585,8 @@ int tp_stage_weights_batched(const tp_stage_item* items, int n_items, int table_
   if (!table_cached)   // pageable source: staged by the runtime before returning (not capturable: cache the table first)
     TP_CUDA_CHECK(cudaMemcpyAsync(d_items, h.data(), sizeof(StageItem) * n_items, cudaMemcpyHostToDevice, st));
   if (kmask_all && kmask_bytes) TP_CUDA_CHECK(cudaMemsetAsync(kmask_all, 0, kmask_bytes, st));   // all layers' occupancy masks: one memset node
-  launch(k_stage_weights_batched, (unsigned)cta, 256, smem, st, d_items, n_items);
+  if (f32) launch(k_stage_weights_batched<float>, (unsigned)cta, 256, smem, st, d_items, n_items);
+  else launch(k_stage_weights_batched<__nv_bfloat16>, (unsigned)cta, 256, smem, st, d_items, n_items);
   if (kmask_all && kmask_bytes) launch(k_kmask_summary, n_items, 256, 0, st, d_items, n_items);
   TP_LAUNCH_CHECK();
   return TP_OK;
@@ -496,6 +601,48 @@ int tp_to_nhwc_bf16(const void* src, int src_dtype, int64_t sn, int64_t sc, int6
   if (src_dtype == 0) launch(k_to_nhwc<float>, grid, 256, 0, st, (const float*)src, sn, sc, sh, sw, n, c, h, w, (__nv_bfloat16*)dst, c_pad);
   else if (src_dtype == 1) launch(k_to_nhwc<__nv_bfloat16>, grid, 256, 0, st, (const __nv_bfloat16*)src, sn, sc, sh, sw, n, c, h, w, (__nv_bfloat16*)dst, c_pad);
   else return TP_ERR_INVALID;
+  TP_LAUNCH_CHECK();
+  return TP_OK;
+}
+
+int tp_to_nhwc_f32(const void* src, int64_t sn, int64_t sc, int64_t sh, int64_t sw,
+                   int n, int c, int h, int w, void* dst, int c_pad, void* stream) {
+  if (!src || !dst || n <= 0 || c <= 0 || h <= 0 || w <= 0 || c_pad < c) return TP_ERR_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long total = (long long)n * h * w * c_pad;
+  const unsigned grid = (unsigned)min((total + 255) / 256, (long long)sm_count() * 32);
+  launch(k_to_nhwc_f32, grid, 256, 0, st, (const float*)src, sn, sc, sh, sw, n, c, h, w, (float*)dst, c_pad);
+  TP_LAUNCH_CHECK();
+  return TP_OK;
+}
+
+int tp_wgrad_split3(const void* src, int64_t sn, int64_t sc, int64_t sh, int64_t sw,
+                    int n, int c, int h, int w, void* dst, int c_pad, int lo_block, void* stream) {
+  if (!src || !dst || n <= 0 || c <= 0 || h <= 0 || w <= 0 || c_pad < c || lo_block < 0 || lo_block > 2) return TP_ERR_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long total = (long long)n * h * w * c_pad;
+  const unsigned grid = (unsigned)min((total + 255) / 256, (long long)sm_count() * 32);
+  launch(k_wgrad_split3, grid, 256, 0, st, (const float*)src, sn, sc, sh, sw, n, c, h, w, (__nv_bfloat16*)dst, c_pad, lo_block);
+  TP_LAUNCH_CHECK();
+  return TP_OK;
+}
+
+int tp_im2col_stem_f32(const void* src, int64_t sn, int64_t sc, int64_t sh, int64_t sw,
+                       int n, int c, int h, int w, int r, int s, int cg, int stride_h, int stride_w, int pad_h, int pad_w,
+                       int p, int q, void* xcol, int kp, void* stream) {
+  if (!src || !xcol || n <= 0 || c <= 0 || c > 8 || cg < c || cg > 8 || kp % 8 != 0 || kp < r * s * cg) return TP_ERR_INVALID;
+  if (r > 255 || s > 255 || kp > 8192) return TP_ERR_UNSUPPORTED;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int QS = q < 128 ? q : 128;
+  const int pw = (QS - 1) * stride_w + s;
+  const size_t patch = ((size_t)r * pw * c + 8) * sizeof(float);
+  if (patch > 80 * 1024 || kp / 8 > 256) return TP_ERR_UNSUPPORTED;
+  if (patch > 48 * 1024)
+    TP_CUDA_CHECK(cudaFuncSetAttribute(k_im2col_stem_rows<float, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)patch));
+  const long long strips = (long long)n * p * ((q + QS - 1) / QS);
+  const unsigned g2 = (unsigned)min(strips, (long long)sm_count() * 8);
+  launch(k_im2col_stem_rows<float, float>, g2, 256, patch, st, (const float*)src, sn, sc, sh, sw, n, c, h, w, r, s, cg, stride_h,
+         stride_w, pad_h, pad_w, p, q, QS, (uint4*)xcol, kp / 8);
   TP_LAUNCH_CHECK();
   return TP_OK;
 }

@@ -35,10 +35,18 @@ def drop_partials():
     _PARTIALS.clear()
 
 
+def fused_enabled():
+    """The fused NHWC kernels are bf16-only: inside ``ops.compute_precision(torch.float32)`` the modules of this file run
+    the reference's own ATen ops (BatchNorm, ReLU, the residual add, max-pool) on the fp32 channels_last activations."""
+    return ops.current_precision() != torch.float32
+
+
 class _BNFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, residual, weight, bias, running_mean, running_var, nbt, momentum, eps, training, relu, grad_slots=None, ext_stats=None,
                 saved=None):
+        if ops.current_precision() == torch.float32:
+            raise RuntimeError("fused BatchNorm is bf16-only: at float32 BatchNorm2dB200 runs ATen's batch_norm")
         lib = _cabi.load()
         ctx.set_materialize_grads(False)
         ctx.grad_slots = grad_slots
@@ -120,7 +128,7 @@ class BatchNorm2dB200(nn.BatchNorm2d):
         training = self.training or not self.track_running_stats
         # eval-mode BN inside an autograd graph is not on the hot path: leave it to torch
         # momentum=None means a cumulative moving average in torch (factor 1/num_batches_tracked): not on the hot path
-        if (not x.is_cuda or x.shape[1] % 8 != 0 or (not training and torch.is_grad_enabled() and x.requires_grad)
+        if (not x.is_cuda or not fused_enabled() or x.shape[1] % 8 != 0 or (not training and torch.is_grad_enabled() and x.requires_grad)
                 or (self.momentum is None and training and self.track_running_stats)):
             y = super().forward(x)
             if residual is not None:
@@ -185,7 +193,7 @@ class MaxPool2dB200(nn.MaxPool2d):
     def forward(self, x):
         k, s, p = self.kernel_size, self.stride, self.padding
         simple = all(isinstance(v, int) for v in (k, s, p)) and self.dilation == 1 and not self.ceil_mode and not self.return_indices
-        if not (simple and x.is_cuda and x.dim() == 4 and x.shape[1] % 8 == 0 and k * k <= 255):
+        if not (simple and x.is_cuda and fused_enabled() and x.dim() == 4 and x.shape[1] % 8 == 0 and k * k <= 255):
             return super().forward(x)
         return _MaxPoolFn.apply(x, k, s, p)
 
@@ -194,7 +202,7 @@ class MaxPool2dB200(nn.MaxPool2d):
 def _stats_ok(conv, bn, x):
     """conv -> bn can hand the batch statistics over through the conv epilogue (training-mode fused BN on CUDA)."""
     from .utils.mask_layers import ConvMask
-    return (isinstance(conv, ConvMask) and isinstance(bn, BatchNorm2dB200) and x.is_cuda and conv.out_channels % 8 == 0
+    return (isinstance(conv, ConvMask) and isinstance(bn, BatchNorm2dB200) and x.is_cuda and fused_enabled() and conv.out_channels % 8 == 0
             and (bn.training or not bn.track_running_stats) and not isinstance(conv.padding, str))
 
 
@@ -205,7 +213,7 @@ def _conv_bn(conv, bn, x, residual=None, relu=False, skip=False):
     xs = x
     if skip:
         from .utils.mask_layers import ConvMask
-        skip = isinstance(conv, ConvMask) and x.requires_grad and x.shape[1] % 64 == 0
+        skip = isinstance(conv, ConvMask) and x.requires_grad and x.shape[1] % 64 == 0 and fused_enabled()
     if fuse:
         outs = conv(x, want_skip=skip, want_stats=True)
         y, stats = outs[0], outs[-1]

@@ -116,24 +116,33 @@ class BaseHarness:
         store.zero()                       # one memset of the persistent gradient storage (param.grad views its slot)
         if self.distributed:
             store.arm()                    # finished gradients start their bucket's reduce on a side stream
-        self._weight_stager().stage()      # bf16(mask * w) operands of every masked layer: one launch
-        with autocast(device_type="cuda", dtype=self.precision, enabled=self.use_amp):
-            outputs = self.model(inputs)
-            loss = self.criterion(outputs, targets)
-        side_wgrad = bool(getattr(self.cfg.experiment_params, "wgrad_side_stream", True))
-        ops.set_wgrad_side_stream(side_wgrad)     # weight gradients run on a side stream beside the dgrad chain ...
-        try:
-            loss.backward()
-        finally:
-            ops.set_wgrad_side_stream(False)
-            ops.join_wgrad(self.device)           # ... and are joined before anything reads param.grad
-            from .. import fused_norm
-            fused_norm.drop_partials()
+        with self._compute_precision():
+            self._weight_stager().stage()      # bf16(mask * w) operands of every masked layer: one launch
+            with autocast(device_type="cuda", dtype=self.precision, enabled=self.use_amp):
+                outputs = self.model(inputs)
+                loss = self.criterion(outputs, targets)
+            side_wgrad = bool(getattr(self.cfg.experiment_params, "wgrad_side_stream", True))
+            ops.set_wgrad_side_stream(side_wgrad)     # weight gradients run on a side stream beside the dgrad chain ...
+            try:
+                loss.backward()
+            finally:
+                ops.set_wgrad_side_stream(False)
+                ops.join_wgrad(self.device)           # ... and are joined before anything reads param.grad
+                from .. import fused_norm
+                fused_norm.drop_partials()
         if self.distributed:
             self.reducer.reduce()          # joins the side stream; leftover buckets go out here
         self.optimizer.step()
         self.train_accuracy.update(outputs.detach(), targets)
         return loss.detach()
+
+    def _compute_precision(self):
+        """training_precision: float32 runs the masked layers with fp32 operands on TF32 tensor cores (the reference's
+        float32 mode with allow_tf32); every other precision keeps the default bf16 kernels."""
+        if self.precision == torch.float32:
+            from .. import ops
+            return ops.compute_precision(torch.float32)
+        return nullcontext()
 
     def _graph_enabled(self):
         return bool(getattr(self.cfg.experiment_params, "cuda_graph", True)) and hasattr(self.optimizer, "sync_lr")
@@ -141,7 +150,7 @@ class BaseHarness:
     def _graph_key(self, inputs, targets):
         from ..utils import mask_layers
         return (tuple(inputs.shape), inputs.dtype, tuple(inputs.stride()), tuple(targets.shape), targets.dtype,
-                id(self.optimizer), self.model.training, mask_layers.mask_epoch())
+                id(self.optimizer), self.model.training, mask_layers.mask_epoch(), self.precision)
 
     def train_step(self, batch):
         """One optimisation step; returns ``{"loss": 0-dim device tensor}`` (the host sync of the reference's
@@ -213,7 +222,7 @@ class BaseHarness:
     def test_step(self, batch):
         inputs, targets = batch
         inputs, targets = inputs.to(self.device, non_blocking=True), targets.to(self.device, non_blocking=True)
-        with torch.no_grad(), autocast(device_type="cuda", dtype=self.precision, enabled=self.use_amp):
+        with torch.no_grad(), self._compute_precision(), autocast(device_type="cuda", dtype=self.precision, enabled=self.use_amp):
             outputs = self.model(inputs)
             loss = self.criterion(outputs, targets)
             self.test_accuracy.update(outputs, targets)

@@ -3,6 +3,8 @@ arithmetic is ours).  Every function here launches hand-written sm_90a kernels t
 ``_cabi`` — there is no eager / CPU fallback.
 """
 import ctypes
+import threading
+from contextlib import contextmanager
 from ctypes import c_void_p
 
 import torch
@@ -10,6 +12,34 @@ import torch
 from . import _cabi
 
 _launches = 0          # number of OUR kernel-launching C-ABI calls (bench.py reports it)
+
+
+# ---- compute precision of the masked layers ---------------------------------------------------------------------------
+# bf16 (the default): bf16 operands and activations, as under the reference's bf16 autocast.  float32: fp32 activations,
+# gradients and operands end to end, GEMMs on TF32 tensor cores — the reference's training_precision: float32 with
+# allow_tf32 = True.  Thread-local like autocast; a masked layer reads it once in its forward and records it for its
+# backward (autograd runs backward on its own thread, where the context is not set).
+_precision = threading.local()
+
+
+def current_precision():
+    return getattr(_precision, "dtype", torch.bfloat16)
+
+
+@contextmanager
+def compute_precision(dtype):
+    """Run the masked layers (and ``WeightStager.stage``) inside this block at ``dtype``: torch.bfloat16 or torch.float32."""
+    if dtype not in (torch.bfloat16, torch.float32):
+        raise ValueError(f"compute_precision: bfloat16 or float32, not {dtype}")
+    prev = getattr(_precision, "dtype", None)
+    _precision.dtype = dtype
+    try:
+        yield
+    finally:
+        if prev is None:
+            del _precision.dtype
+        else:
+            _precision.dtype = prev
 
 
 def _count(n=1):
@@ -479,12 +509,55 @@ class WeightStager:
             lib = _cabi.load()
             self._ws = torch.empty(max(int(lib.tp_stage_batched_workspace_bytes(len(self.layers))), 256), dtype=torch.uint8, device=dev)
 
+    def _stage_f32(self, key):
+        """fp32 operands (inside ``compute_precision(torch.float32)``): the same layouts as fp32, their own persistent
+        buffers and pointer table, no occupancy masks."""
+        lib = _cabi.load()
+        st = self.__dict__.setdefault("_f32", {})
+        if st.get("key") != key:
+            dev = self.layers[0].weight.device
+            if "bufs" not in st:
+                bufs = []
+                for l in self.layers:
+                    cout, cin, r, s = self._shape4(l)
+                    if not l.weight.is_cuda or l.weight.dtype != torch.float32 or not l.weight.is_contiguous():
+                        bufs.append(None); continue
+                    cin_p, cout_p, has_wd, wf_ld = _operand_plan(cout, cin, r, s)
+                    wf = torch.zeros(cout, wf_ld, dtype=torch.float32, device=dev)
+                    wd = torch.zeros(cin, r * s * cout_p, dtype=torch.float32, device=dev) if has_wd else None
+                    bufs.append((wf, wd, cin_p, cout_p))
+                st["bufs"] = bufs
+                st["ws"] = torch.empty(max(int(lib.tp_stage_batched_workspace_bytes(len(self.layers))), 256), dtype=torch.uint8,
+                                       device=dev)
+            live = [(l, b) for l, b in zip(self.layers, st["bufs"]) if b is not None]
+            items = (_cabi.StageItem * len(live))()
+            for it, (l, (wf, wd, cin_p, cout_p)) in zip(items, live):
+                cout, cin, r, s = self._shape4(l)
+                it.w = l.weight.data_ptr(); it.mask = l.mask.data_ptr()
+                it.wf = wf.data_ptr(); it.wd = wd.data_ptr() if wd is not None else None
+                it.cout, it.cin, it.r, it.s, it.cin_p, it.cout_p, it.wf_ld = cout, cin, r, s, cin_p, cout_p, wf.shape[1]
+                it.kmask_f = it.kmask_d = None
+            st.update(key=key, items=items, live=live, cached=False)
+        if not st["live"]:
+            return
+        dev = self.layers[0].weight.device
+        with torch.cuda.device(dev):
+            rc = lib.tp_stage_weights_batched_f32(st["items"], len(st["live"]), int(st["cached"]), c_void_p(st["ws"].data_ptr()),
+                                                  st["ws"].numel(), _cabi.stream_ptr(dev))
+        _cabi.check(rc, "tp_stage_weights_batched_f32")
+        st["cached"] = True
+        _count()
+        for l, (wf, wd, _, _) in st["live"]:
+            l.__dict__["_tp_staged"] = (wf, wd)
+
     def stage(self):
         lib = _cabi.load()
         for l in self.layers:                                  # masks created on the host move with the first use
             if l.mask.device != l.weight.device or l.mask.dtype != torch.float32 or not l.mask.is_contiguous():
                 l.mask = l.mask.to(device=l.weight.device, dtype=torch.float32).contiguous()
         key = tuple((l.weight.data_ptr(), l.mask.data_ptr()) for l in self.layers)
+        if current_precision() == torch.float32:
+            return self._stage_f32(key)
         cached = key == self._key
         if not cached:
             self._rebuild(key)
@@ -516,10 +589,13 @@ def skipped_block_report(stager):
 
 
 def take_staged(layer):
-    """The (wf, wd) pair a ``WeightStager`` left for this layer's next forward, or None; consumed exactly once."""
+    """The (wf, wd) pair a ``WeightStager`` left for this layer's next forward, or None; consumed exactly once.  A pair
+    staged at the other precision than the current one is dropped."""
     st = layer.__dict__.get("_tp_staged")
     if st is not None:
         layer.__dict__["_tp_staged"] = None
+        if st[0].dtype != (torch.float32 if current_precision() == torch.float32 else torch.bfloat16):
+            return None
     return st
 
 
@@ -554,10 +630,10 @@ def im2col_c8(x_nhwc8, desc, kp):
     return out
 
 
-def empty_cl(n, c, h, w, device):
+def empty_cl(n, c, h, w, device, dtype=torch.bfloat16):
     """[n, c, h, w] bf16 with channels_last strides: the memory IS an NHWC array, and the tensor is not a view
     (autograd forbids in-place ops such as nn.ReLU(inplace=True) on views created inside a custom Function)."""
-    return torch.empty((n, c, h, w), dtype=torch.bfloat16, device=device, memory_format=torch.channels_last)
+    return torch.empty((n, c, h, w), dtype=dtype, device=device, memory_format=torch.channels_last)
 
 
 def im2col_stem(x, desc, kp, cg):
@@ -666,6 +742,228 @@ def conv_wgrad(desc, x_nhwc, dy_nhwc, mask4d, cin_real, want_db=False, dw_out=No
     return dw, db
 
 
+# ---- fp32 (TF32) masked layers: inside compute_precision(torch.float32) ------------------------------------------------
+def stage_weights_f32(weight4d, mask4d, cin_p, need_dgrad, cout_p=None, wf_ld=0):
+    """fp32 mask*w in the layouts of ``stage_weights`` (no occupancy masks)."""
+    lib = _cabi.load()
+    cout, cin, r, s = weight4d.shape
+    dev = weight4d.device
+    wf = torch.zeros(cout, wf_ld, dtype=torch.float32, device=dev) if wf_ld and wf_ld > r * s * cin_p else \
+        torch.empty(cout, r * s * cin_p, dtype=torch.float32, device=dev)
+    cout_p = cout if cout_p is None else cout_p
+    wd = torch.empty(cin, r * s * cout_p, dtype=torch.float32, device=dev) if need_dgrad else None
+    with torch.cuda.device(dev):
+        rc = lib.tp_stage_weights_f32(c_void_p(weight4d.data_ptr()), c_void_p(mask4d.data_ptr()), cout, cin, r, s,
+                                      c_void_p(wf.data_ptr()), cin_p, int(wf_ld), c_void_p(wd.data_ptr()) if wd is not None else None,
+                                      cout_p, _cabi.stream_ptr(dev))
+    _cabi.check(rc, "tp_stage_weights_f32")
+    _count()
+    return wf, wd
+
+
+def to_nhwc_f32(x, c_pad):
+    """[N, C, H, W] fp32 (any strides) -> NHWC fp32 [N, H, W, c_pad]: a view when x already is channels_last with C == c_pad."""
+    n, c, h, w = x.shape
+    if x.dtype != torch.float32:
+        raise TypeError(f"to_nhwc_f32: fp32 input expected, got {x.dtype}")
+    if c == c_pad and x.permute(0, 2, 3, 1).is_contiguous():
+        return x.permute(0, 2, 3, 1)
+    lib = _cabi.load()
+    out = torch.empty(n, h, w, c_pad, dtype=torch.float32, device=x.device)
+    sn, sc, sh, sw = x.stride()
+    with torch.cuda.device(x.device):
+        rc = lib.tp_to_nhwc_f32(c_void_p(x.data_ptr()), sn, sc, sh, sw, n, c, h, w, c_void_p(out.data_ptr()), c_pad,
+                                _cabi.stream_ptr(x.device))
+    _cabi.check(rc, "tp_to_nhwc_f32")
+    _count()
+    return out
+
+
+def im2col_stem_f32(x, desc, kp, cg):
+    """[N, C<=8, H, W] fp32 (any strides) -> [N*P*Q, kp] fp32 im2col matrix (the layout of ``im2col_stem``)."""
+    lib = _cabi.load()
+    n, c, h, w = x.shape
+    out = torch.empty(n * desc.p * desc.q, kp, dtype=torch.float32, device=x.device)
+    sn, sc, sh, sw = x.stride()
+    with torch.cuda.device(x.device):
+        rc = lib.tp_im2col_stem_f32(c_void_p(x.data_ptr()), sn, sc, sh, sw, n, c, h, w, desc.r, desc.s, cg, desc.stride_h,
+                                    desc.stride_w, desc.pad_h, desc.pad_w, desc.p, desc.q, c_void_p(out.data_ptr()), kp,
+                                    _cabi.stream_ptr(x.device))
+    _cabi.check(rc, "tp_im2col_stem_f32")
+    _count()
+    return out
+
+
+def conv_fprop_f32(desc, x_nhwc, wf, bias=None, out=None):
+    lib = _cabi.load()
+    dev = x_nhwc.device
+    y = out if out is not None else torch.empty(desc.n, desc.p, desc.q, desc.cout, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev), _Timed("fprop", desc):
+        rc = lib.tp_conv_fprop_f32(ctypes.byref(desc), c_void_p(x_nhwc.data_ptr()), c_void_p(wf.data_ptr()),
+                                   c_void_p(bias.data_ptr()) if bias is not None else None, c_void_p(y.data_ptr()),
+                                   _cabi.stream_ptr(dev))
+    _cabi.check(rc, "tp_conv_fprop_f32")
+    _count()
+    return y
+
+
+def conv_dgrad_f32(desc, dy_nhwc, wd):
+    lib = _cabi.load()
+    dev = dy_nhwc.device
+    dx = torch.empty(desc.n, desc.h, desc.w, desc.cin, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev), _Timed("dgrad", desc):
+        rc = lib.tp_conv_dgrad_f32(ctypes.byref(desc), c_void_p(dy_nhwc.data_ptr()), c_void_p(wd.data_ptr()),
+                                   c_void_p(dx.data_ptr()), _cabi.stream_ptr(dev))
+    _cabi.check(rc, "tp_conv_dgrad_f32")
+    _count()
+    return dx
+
+
+def wgrad_split3(x, c_pad, lo_block):
+    """fp32 [N, C, H, W] (any strides) -> NHWC bf16 [3N, H, W, c_pad]: image block ``lo_block`` holds bf16(v - bf16(v)),
+    the other two bf16(v) (see ``conv_wgrad_f32``)."""
+    lib = _cabi.load()
+    n, c, h, w = x.shape
+    out = torch.empty(3 * n, h, w, c_pad, dtype=torch.bfloat16, device=x.device)
+    sn, sc, sh, sw = x.stride()
+    with torch.cuda.device(x.device):
+        rc = lib.tp_wgrad_split3(c_void_p(x.data_ptr()), sn, sc, sh, sw, n, c, h, w, c_void_p(out.data_ptr()), c_pad, int(lo_block),
+                                 _cabi.stream_ptr(x.device))
+    _cabi.check(rc, "tp_wgrad_split3")
+    _count()
+    return out
+
+
+def split_stacks(desc, x, dy, dy_c_pad):
+    """The bf16 stacks of the fp32 weight gradient: x [N, cin, H, W] as (hi, lo, hi), dy [N, cout, P, Q] as (hi, hi, lo)."""
+    return wgrad_split3(x, desc.cin, 1), wgrad_split3(dy, dy_c_pad, 2)
+
+
+def conv_wgrad_f32(desc, xs, dys, mask4d, cin_real, dw_out=None):
+    """fp32 masked weight gradient from the stacks of ``split_stacks``: ONE bf16 ``conv_wgrad`` over 3N images sums
+    x_hi dy_hi + x_lo dy_hi + x_hi dy_lo in its deterministic split-K fold (TF32 wgmma cannot read the MN-major operands
+    of the pixel contraction).  hi + lo carries 16 significant bits, so each product is within about 2^-16 relative
+    (the dropped x_lo dy_lo term and the rounding of lo) — closer than TF32's 2^-10 per operand.  No bias gradient here:
+    the stacked column sum would count dy_hi twice."""
+    d3 = _cabi.ConvDesc(3 * desc.n, desc.h, desc.w, desc.cin, desc.cout, desc.r, desc.s, desc.stride_h, desc.stride_w,
+                        desc.pad_h, desc.pad_w, desc.p, desc.q)
+    dw, _ = conv_wgrad(d3, xs, dys, mask4d, cin_real, False, dw_out=dw_out)
+    return dw
+
+
+def _fp32_forward(ctx, x, weight, mask, bias, stride, padding, want_skip, grad_slots, staged, want_stats):
+    if want_skip or want_stats:
+        raise RuntimeError("masked_conv2d at float32: the skip-gradient and BatchNorm-statistics epilogues exist in bf16 "
+                           "only (a float32 model runs unfused)")
+    if x.dtype != torch.float32:
+        raise TypeError(f"masked layers at float32 need fp32 activations, got {x.dtype}")
+    ctx.set_materialize_grads(False)
+    ctx.f32 = True
+    ctx.grad_slots = grad_slots
+    cout, cin, r, s = weight.shape
+    n, _, h, w = x.shape
+    need_dx = ctx.needs_input_grad[0]
+    w32 = weight.detach().contiguous()
+    m32 = mask.detach().contiguous()
+    cin_p = padded_cin(cin, r, s)
+    small_c = cin <= 8 and cin_p != cin and not need_dx
+    desc = make_desc(n, h, w, cin_p if not small_c else cin, cout, r, s, stride, padding)
+    cout_p = _round_up(cout, 64 if (r * s > 1 and not small_c) else 8)
+    y = empty_cl(n, cout, desc.p, desc.q, x.device, torch.float32)
+    if small_c:
+        cg, kp = stem_geometry(cin, r, s)
+        xg = im2col_stem_f32(x, desc, kp, cg)
+        gdesc = _cabi.ConvDesc(n * desc.p * desc.q, 1, 1, kp, cout, 1, 1, 1, 1, 0, 0, 1, 1)
+        wf = staged[0] if staged is not None and staged[0].shape == (cout, kp) else stage_weights_f32(w32, m32, cg, False, wf_ld=kp)[0]
+        conv_fprop_f32(gdesc, xg, wf, bias, out=y)
+        ctx.mode = "stem"
+        ctx.gdesc = gdesc
+        ctx.save_for_backward(xg, m32)
+    else:
+        xn = to_nhwc_f32(x, cin_p)
+        if (staged is not None and staged[0].shape == (cout, r * s * cin_p)
+                and (not need_dx or (staged[1] is not None and staged[1].shape == (cin, r * s * cout_p)))):
+            wf, wd = staged
+        else:
+            wf, wd = stage_weights_f32(w32, m32, cin_p, need_dx, cout_p)
+        conv_fprop_f32(desc, xn, wf, bias, out=y)
+        ctx.mode = "conv"
+        ctx.save_for_backward(xn, m32, wd)
+    ctx.desc = desc
+    ctx.cin = cin
+    ctx.has_bias = bias is not None
+    ctx.cout_p = cout_p
+    return y
+
+
+def _fp32_backward(ctx, dy):
+    desc = ctx.desc
+    rest = (None,) * 7                      # stride, padding, want_skip, grad_slots, staged, want_stats, bn_src
+    if dy is None:
+        return (None, None, None, None) + rest
+    cout = desc.cout
+    need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+    need_db = ctx.has_bias and ctx.needs_input_grad[3]
+    if dy.dtype != torch.float32:
+        dy = dy.float()
+    dx = dw = db = None
+    if ctx.mode == "stem":
+        xg, m32 = ctx.saved_tensors
+        if need_dw:
+            r, s = desc.r, desc.s
+            cin = m32.shape[1]
+            rows, kp = xg.shape
+            gd = ctx.gdesc
+            # dy [N, cout, P, Q] splits to NHWC [3N, P, Q, cout]: the rows of the im2col matrix, three times over
+            xs, dys = split_stacks(gd, xg.view(rows, kp, 1, 1), dy, cout)
+            ones = torch.ones(cout, kp, dtype=torch.float32, device=xg.device)
+            dwm = conv_wgrad_f32(gd, xs, dys, ones.view(cout, kp, 1, 1), kp)
+            cg = stem_geometry(cin, r, s)[0]
+            dw = dwm[:, :r * s * cg].reshape(cout, r * s, cg)[:, :, :cin].permute(0, 2, 1).reshape(cout, cin, r, s) * m32
+    else:
+        xn, m32, wd = ctx.saved_tensors
+        cin = ctx.cin
+        ddesc = desc
+        if ctx.cout_p != cout:
+            ddesc = _cabi.ConvDesc(desc.n, desc.h, desc.w, desc.cin, ctx.cout_p, desc.r, desc.s, desc.stride_h,
+                                   desc.stride_w, desc.pad_h, desc.pad_w, desc.p, desc.q)
+        if need_dx:
+            dyn = to_nhwc_f32(dy, ctx.cout_p)
+            xdesc = ddesc if cin == desc.cin else _cabi.ConvDesc(desc.n, desc.h, desc.w, cin, ctx.cout_p, desc.r, desc.s,
+                                                                  desc.stride_h, desc.stride_w, desc.pad_h, desc.pad_w,
+                                                                  desc.p, desc.q)
+            dx = conv_dgrad_f32(xdesc, dyn, wd).permute(0, 3, 1, 2)
+        if need_dw:
+            # the stacks are written on the current stream; the GEMM may run on the side stream, which then owns them
+            xs, dys = split_stacks(ddesc, xn.permute(0, 3, 1, 2), dy, ctx.cout_p)
+            if ctx.cout_p != cout:
+                m_p = torch.zeros(ctx.cout_p, *m32.shape[1:], dtype=torch.float32, device=m32.device)
+                m_p[:cout] = m32
+                dw = conv_wgrad_f32(ddesc, xs, dys, m_p, cin)[:cout].contiguous()
+            else:
+                ws_ = ctx.grad_slots[0] if ctx.grad_slots is not None else None
+                direct_w = ws_ is not None and ws_.is_contiguous() and ws_.numel() == m32.numel()
+                if WGRAD_SIDE_STREAM and direct_w:
+                    dev = xn.device
+                    cur, side = torch.cuda.current_stream(dev), _wgrad_stream(dev)
+                    ev = torch.cuda.Event(); ev.record(cur)
+                    side.wait_event(ev)
+                    with torch.cuda.stream(side):
+                        conv_wgrad_f32(desc, xs, dys, m32, cin, dw_out=ws_)
+                        grad_ready(ws_)
+                    # freed as soon as this layer's GEMM is done, not at the join: 6 B per element of x and dy
+                    xs.record_stream(side); dys.record_stream(side); m32.record_stream(side)
+                    _wgrad_keepalive.append((ws_,))        # join_wgrad() waits for the side stream while anything is pending
+                else:
+                    dw = conv_wgrad_f32(desc, xs, dys, m32, cin, dw_out=ws_ if direct_w else None)
+                    if direct_w:
+                        dw = None
+                        grad_ready(ws_)
+    if need_db:
+        db = dy.sum(dim=(0, 2, 3))
+    return (dx, dw, None, db) + rest
+
+
 class MaskedConv2dFn(torch.autograd.Function):
     """y = conv2d(x, mask*w, b) with bf16 tensor-core operands and fp32 accumulation.
 
@@ -679,6 +977,8 @@ class MaskedConv2dFn(torch.autograd.Function):
     def forward(ctx, x, weight, mask, bias, stride, padding, want_skip=False, grad_slots=None, staged=None, want_stats=False,
                 bn_src=None):
         _require_cuda(x, weight, mask)
+        if current_precision() == torch.float32:        # read once; backward follows ctx.f32
+            return _fp32_forward(ctx, x, weight, mask, bias, stride, padding, want_skip, grad_slots, staged, want_stats)
         ctx.set_materialize_grads(False)
         ctx.bn_src = None
         ctx.want_skip = want_skip
@@ -757,6 +1057,8 @@ class MaskedConv2dFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dy, *rest):
+        if getattr(ctx, "f32", False):
+            return _fp32_backward(ctx, dy)
         # outputs were (y [, x_skip] [, stats]); the statistics output is non-differentiable
         dskip = rest[0] if ctx.want_skip and rest else None
         desc = ctx.desc

@@ -140,6 +140,8 @@ class TorchVisionModel(PruneModel):
         self._replace_layers()
         # BatchNorm / ReLU / residual-add between the masked convs run as fused NHWC kernels
         # (same modules, parameters and state-dict keys; SURVEY.md §8(f) row 1).
+        # Inside ops.compute_precision(torch.float32) (a float32 config's step) these modules run the reference's own
+        # ATen ops instead: the fused kernels are bf16-only (fused_norm.fused_enabled).
         if getattr(cfg.model_params, "fuse_norm", True):
             from ..fused_norm import fuse_torchvision_blocks
             fuse_torchvision_blocks(self.model)

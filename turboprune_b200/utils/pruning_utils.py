@@ -15,6 +15,7 @@ Things kept on purpose:
     order, because the RNG stream is part of mask parity (:112, :314; mask_layers.py:43);
   * an unknown method prints an error and returns (:33-37).
 """
+from contextlib import nullcontext
 from typing import Any, List
 
 import torch
@@ -32,6 +33,11 @@ def _masked(model: nn.Module) -> List[nn.Module]:
 def get_dtype_amp(cfg):
     table = {"bfloat16": (torch.bfloat16, True), "float16": (torch.float16, True), "float32": (torch.float32, False)}
     return table.get(cfg.experiment_params.training_precision, (torch.float32, False))
+
+
+def _compute_precision(precision):
+    """float32 configs score with fp32 activations and gradients (TF32 GEMMs); the others with the default bf16 kernels."""
+    return ops.compute_precision(torch.float32) if precision == torch.float32 else nullcontext()
 
 
 def _global_prune(model: nn.Module, density: float, kind: int) -> nn.Module:
@@ -61,7 +67,7 @@ def prune_snip(cfg, model: nn.Module, trainloader: Any, density: float) -> nn.Mo
     for images, target in trainloader:
         images = images.to(dev)
         target = target.to(dev).long()
-        with autocast("cuda", dtype=precision, enabled=use_amp):
+        with _compute_precision(precision), autocast("cuda", dtype=precision, enabled=use_amp):
             model.zero_grad()
             criterion(model(images), target).backward()
         break
@@ -84,7 +90,7 @@ def prune_synflow(cfg, model: nn.Module, trainloader: Any, density: float) -> nn
     for images, _ in trainloader:
         shape = [1] + list(images[0, :].shape)
         ones = torch.ones(shape, device=dev)
-        with autocast("cuda", dtype=precision, enabled=use_amp):
+        with _compute_precision(precision), autocast("cuda", dtype=precision, enabled=use_amp):
             torch.sum(model(ones)).backward()
         break
     layers = _masked(model)
