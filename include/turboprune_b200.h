@@ -95,6 +95,27 @@ int tp_apply_threshold(const void* const* w, const void* const* g, const void* c
 int tp_count_zeros(const void* const* m, const int64_t* numel, int n_seg,
                    int64_t* zeros_out, void* ws, size_t ws_bytes, void* stream);
 
+/* ---- RigL drop-and-regrow (dynamic sparse training, Evci et al. 2020) -------------------
+ * tp_rigl_select: for every segment (layer) i at once, exact and deterministic:
+ *   DROP  among the positions with mask != 0, the k[i] smallest |w|;
+ *   GROW  among the positions with mask == 0 after the drop (just-dropped ones included), the k[i] largest |g|.
+ * Order: the fp32 bit pattern of |x| (sign bit cleared) as an unsigned integer, so NaN sorts above +inf; ties go to
+ * the lower flat index first.  k[i] larger than the active count drops all of them; the grow always takes as many as
+ * the drop took, so every segment keeps its active count.
+ *   w, g, mask, new_mask_out : HOST arrays of n_seg DEVICE pointers (fp32); new_mask_out gets the 0/1 mask after
+ *                              the update (mask itself is not written)
+ *   numel, k                 : HOST int64 arrays; numel[i] <= 2^31, k[i] >= 0
+ *   counts_out               : DEVICE int64 [n_seg][2] = (dropped, grown), counted from the masks written
+ * No host synchronisation.  Workspace: tp_rigl_workspace_bytes(n_seg, sum numel). */
+size_t tp_rigl_workspace_bytes(int n_seg, int64_t total_numel);
+int tp_rigl_select(const void* const* w, const void* const* g, const void* const* mask, void* const* new_mask_out,
+                   const int64_t* numel, const int64_t* k, int n_seg, int64_t* counts_out, void* ws, size_t ws_bytes,
+                   void* stream);
+/* mask <- new_mask in place; where new_mask != 0 and mask == 0 the weight and its momentum restart from 0 (momentum[i]
+ * or the whole array may be NULL).  One launch.  Workspace: tp_segtable_workspace_bytes(n_seg). */
+int tp_rigl_apply(void* const* mask, const void* const* new_mask, void* const* w, void* const* momentum,
+                  const int64_t* numel, int n_seg, void* ws, size_t ws_bytes, void* stream);
+
 /* ---- weight staging: fp32 (mask*w) -> bf16 tensor-core operand layouts ------------------
  * Replaces the per-forward `mask * weight` (utils/mask_layers.py:25,69,109) and the autocast
  * fp32->bf16 cast of the product: one pass writes

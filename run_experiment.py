@@ -20,6 +20,7 @@ from turboprune_b200.harness_definitions.standard_pruning_harness import Pruning
 from turboprune_b200.utils import config as tp_config
 from turboprune_b200.utils.harness_utils import gen_expt_dir, generate_densities, save_config, save_model, set_seed
 from turboprune_b200.utils.pruning_utils import prune_the_model
+from turboprune_b200.utils.rigl import rigl_params
 
 
 def check_replicas(model, what):
@@ -44,6 +45,7 @@ def main(cfg):
             print("CIFAR datasets do not support distributed training. Please run without torchrun/distributed launch.")
         sys.exit(1)                                           # reference run_experiment.py:25-37
     use_distributed = cfg.experiment_params.distributed and not cifar and launched
+    rigl_params(cfg)                                          # a RigL config needs a one-shot initial mask: fail before training
     set_seed(cfg)
     if use_distributed:
         torch.cuda.set_device(int(os.environ["LOCAL_RANK"]))
@@ -62,7 +64,7 @@ def main(cfg):
         packaged = box[0]
     harness = PruningHarness(cfg=cfg, gpu_id=rank, expt_dir=packaged)
     model = harness.model
-    at_init = cfg.pruning_params.training_type == "at_init"
+    at_init = cfg.pruning_params.training_type in ("at_init", "rigl")     # RigL: the one-shot mask at level 0, one level
     densities = generate_densities(cfg=cfg, current_sparsity=model.get_overall_sparsity())
     ckpt = os.path.join(packaged[1], "checkpoints")
     for level, density in enumerate(densities):

@@ -49,6 +49,11 @@ SIGNATURES = {
     "tp_apply_threshold": (c_int, [POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p),
                                    POINTER(c_int64), c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "tp_count_zeros": (c_int, [POINTER(c_void_p), POINTER(c_int64), c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "tp_rigl_workspace_bytes": (c_size_t, [c_int, c_int64]),
+    "tp_rigl_select": (c_int, [POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_int64),
+                               POINTER(c_int64), c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "tp_rigl_apply": (c_int, [POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_int64), c_int,
+                              c_void_p, c_size_t, c_void_p]),
     "tp_stage_weights": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_int,
                                  c_int, c_void_p, c_void_p, c_void_p]),
     "tp_kblock_mask_words": (c_size_t, [c_int64]),

@@ -25,6 +25,7 @@
 // integers; NaN patterns (> 0x7f800000) sort above +inf exactly like ATen's radix key
 // (SortingRadixSelect.cuh:20-39).
 #include "tp_common.cuh"
+#include <vector>
 
 namespace tp {
 
@@ -687,6 +688,311 @@ static int finish_topk(const TopkWs& w, int n_seg, long long tiles, long long k,
   return TP_OK;
 }
 
+// ---------------------------------------------------------------------------------------------
+// RigL drop-and-regrow (Evci et al. 2020), exact per segment (= layer):
+//   DROP: among mask != 0, the k smallest |w|;   GROW: among new mask == 0 after the drop, the k largest |g|.
+// Key: the fp32 bit pattern of |x| (sign cleared) as an unsigned integer; GROW uses its complement, so that both are
+// "k smallest keys".  Ties at the k-th key go to the lower flat index first.  For each of DROP and GROW:
+//   3 x (k_rigl_hist, k_rigl_pick) : 11/11/10-bit radix select on one 2048-bin histogram per segment -> threshold key T
+//                                    and r = how many of the eligible keys == T are taken
+//   k_rigl_ties                    : per tile, the eligible keys == T
+//   k_rigl_tie_scan                : per segment, the exclusive prefix of those counts over its tiles
+//   k_rigl_write                   : selected = key < T, or key == T with index-order rank < r (block prefix in the tile);
+//                                    DROP writes new = (mask != 0) && !selected, GROW sets new = 1 where selected
+// Every thread owns kRiglPer neighbouring elements of a tile, so the block prefix follows the flat index.  Integer
+// atomics only: masks and counts are deterministic.  A k larger than the active count drops all of them; the grow
+// always takes as many as the drop took, so every segment keeps its active count.
+constexpr int kRiglPer = kTileElems / kSweepThreads;      // 16
+
+struct RiglSel {
+  unsigned long long k;          // requested count; after the first pick, min(k, eligible)
+  unsigned long long k_rem;      // ties at the threshold still to take
+  unsigned int prefix, pmask;    // selected digits so far; after three passes prefix is the threshold key T
+  int none;                      // nothing to select in this segment (k == 0 or no eligible position)
+  int pad_;
+};
+
+// Load this thread's kRiglPer elements of a tile: their keys, and a bit per eligible position.
+template <int PHASE>
+__device__ __forceinline__ unsigned int rigl_load(const Seg& sg, long long base, int n_in, unsigned int (&key)[kRiglPer]) {
+  const int j0 = threadIdx.x * kRiglPer;
+  int cnt = n_in - j0;
+  cnt = cnt < 0 ? 0 : (cnt > kRiglPer ? kRiglPer : cnt);
+  const float* a = (PHASE == 0 ? sg.m : sg.mo) + base + j0;     // eligibility operand
+  const float* b = (PHASE == 0 ? sg.w : sg.g) + base + j0;      // key operand
+  float va[kRiglPer], vb[kRiglPer];
+  if (cnt == kRiglPer && ((((uintptr_t)a) | ((uintptr_t)b)) & 15) == 0) {
+#pragma unroll
+    for (int q = 0; q < kRiglPer / 4; ++q) {
+      const float4 x = ((const float4*)a)[q], y = ((const float4*)b)[q];
+      va[4 * q] = x.x; va[4 * q + 1] = x.y; va[4 * q + 2] = x.z; va[4 * q + 3] = x.w;
+      vb[4 * q] = y.x; vb[4 * q + 1] = y.y; vb[4 * q + 2] = y.z; vb[4 * q + 3] = y.w;
+    }
+  } else {
+#pragma unroll
+    for (int j = 0; j < kRiglPer; ++j) { va[j] = j < cnt ? a[j] : 0.f; vb[j] = j < cnt ? b[j] : 0.f; }
+  }
+  unsigned int elig = 0;
+#pragma unroll
+  for (int j = 0; j < kRiglPer; ++j) {
+    const unsigned int mag = __float_as_uint(vb[j]) & 0x7fffffffu;
+    key[j] = PHASE == 0 ? mag : ~mag;
+    const bool e = j < cnt && (PHASE == 0 ? va[j] != 0.f : va[j] == 0.f);
+    elig |= (unsigned int)e << j;
+  }
+  return elig;
+}
+
+__device__ __forceinline__ unsigned int block_sum_u32(unsigned int v, unsigned int* s_red /* [kSweepThreads / 32] */) {
+  for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) s_red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  unsigned int tot = 0;
+#pragma unroll
+  for (int i = 0; i < kSweepThreads / 32; ++i) tot += s_red[i];
+  return tot;
+}
+
+// Exclusive prefix of v over the block in thread order; *total gets the sum.
+__device__ __forceinline__ unsigned int block_excl_scan_u32(unsigned int v, unsigned int* s_red /* [kSweepThreads / 32] */,
+                                                            unsigned int* total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  unsigned int inc = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned int u = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += u;
+  }
+  __syncthreads();
+  if (lane == 31) s_red[warp] = inc;
+  __syncthreads();
+  unsigned int before = 0, tot = 0;
+#pragma unroll
+  for (int i = 0; i < kSweepThreads / 32; ++i) { before += i < warp ? s_red[i] : 0u; tot += s_red[i]; }
+  *total = tot;
+  return before + inc - v;
+}
+
+// One digit pass: per-segment histograms of the eligible keys that match the prefix.  Each CTA walks a contiguous
+// range of tiles and flushes its shared histogram when the segment changes.
+template <int PHASE>
+__global__ void __launch_bounds__(kSweepThreads) k_rigl_hist(const Seg* __restrict__ segs, int n_seg, long long tiles,
+                                                             const RiglSel* __restrict__ sel, int shift, int nbits,
+                                                             unsigned int* __restrict__ hist) {
+  __shared__ unsigned int s_hist[2048];
+  const int t = threadIdx.x;
+  const unsigned int dmask = (1u << nbits) - 1u;
+  for (int i = t; i < 2048; i += kSweepThreads) s_hist[i] = 0;
+  __syncthreads();
+  const long long t0 = tiles * blockIdx.x / gridDim.x, t1 = tiles * (blockIdx.x + 1) / gridDim.x;
+  int cur = -1;
+  bool dirty = false;
+  for (long long tile = t0; tile < t1; ++tile) {
+    const int si = find_seg(segs, n_seg, tile);
+    if (si != cur) {
+      if (dirty) {
+        __syncthreads();
+        for (int i = t; i < 2048; i += kSweepThreads)
+          if (s_hist[i]) { atomicAdd(&hist[(size_t)cur * 2048 + i], s_hist[i]); s_hist[i] = 0; }
+        __syncthreads();
+      }
+      cur = si; dirty = false;
+    }
+    const RiglSel s = sel[si];
+    if (s.none) continue;
+    const Seg sg = segs[si];
+    const long long base = (tile - sg.tile0) * kTileElems;
+    const long long rem = sg.n - base;
+    unsigned int key[kRiglPer];
+    const unsigned int elig = rigl_load<PHASE>(sg, base, rem < kTileElems ? (int)rem : kTileElems, key);
+#pragma unroll
+    for (int j = 0; j < kRiglPer; ++j)
+      if (((elig >> j) & 1u) && (key[j] & s.pmask) == s.prefix) atomicAdd(&s_hist[(key[j] >> shift) & dmask], 1u);
+    dirty = true;
+  }
+  if (dirty) {
+    __syncthreads();
+    for (int i = t; i < 2048; i += kSweepThreads)
+      if (s_hist[i]) atomicAdd(&hist[(size_t)cur * 2048 + i], s_hist[i]);
+  }
+}
+
+// One CTA per segment: pick the digit holding the k_rem-th key, then clear the histogram for the next pass.  The first
+// pass clamps k to the eligible count and, for GROW, to what the DROP took (`cap`, NULL for DROP).
+__global__ void __launch_bounds__(kSweepThreads) k_rigl_pick(unsigned int* __restrict__ hist, RiglSel* __restrict__ sel,
+                                                             const RiglSel* __restrict__ cap, int shift, int nbits, int first) {
+  __shared__ unsigned int s_bin, s_red[kSweepThreads / 32];
+  __shared__ unsigned long long s_before, s_warp[32];
+  const int t = threadIdx.x;
+  RiglSel* s = sel + blockIdx.x;
+  unsigned int* h = hist + (size_t)blockIdx.x * 2048;
+  if (s->none) return;
+  unsigned long long kr = s->k_rem;
+  if (first) {
+    unsigned int loc = 0;
+#pragma unroll
+    for (int i = 0; i < 2048 / kSweepThreads; ++i) loc += h[t * (2048 / kSweepThreads) + i];
+    const unsigned long long eligible = block_sum_u32(loc, s_red);
+    kr = s->k < eligible ? s->k : eligible;
+    if (cap && cap[blockIdx.x].k < kr) kr = cap[blockIdx.x].k;
+    if (kr == 0) {
+      for (int i = t; i < 2048; i += kSweepThreads) h[i] = 0;
+      if (t == 0) { s->k = 0; s->none = 1; }
+      return;
+    }
+  }
+  block_find_rank<2048 / kSweepThreads>(h, kr, &s_bin, &s_before, s_warp);
+  for (int i = t; i < 2048; i += kSweepThreads) h[i] = 0;
+  if (t == 0) {
+    if (first) s->k = kr;
+    s->prefix |= s_bin << shift;
+    s->pmask |= ((1u << nbits) - 1u) << shift;
+    s->k_rem = kr - s_before;
+  }
+}
+
+template <int PHASE>
+__global__ void __launch_bounds__(kSweepThreads) k_rigl_ties(const Seg* __restrict__ segs, int n_seg, long long tiles,
+                                                             const RiglSel* __restrict__ sel, unsigned int* __restrict__ tie_cnt) {
+  __shared__ unsigned int s_red[kSweepThreads / 32];
+  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int si = find_seg(segs, n_seg, tile);
+    const RiglSel s = sel[si];
+    unsigned int c = 0;
+    if (!s.none) {
+      const Seg sg = segs[si];
+      const long long base = (tile - sg.tile0) * kTileElems;
+      const long long rem = sg.n - base;
+      unsigned int key[kRiglPer];
+      const unsigned int elig = rigl_load<PHASE>(sg, base, rem < kTileElems ? (int)rem : kTileElems, key);
+#pragma unroll
+      for (int j = 0; j < kRiglPer; ++j) c += ((elig >> j) & 1u) && key[j] == s.prefix;
+    }
+    const unsigned int tot = block_sum_u32(c, s_red);
+    if (threadIdx.x == 0) tie_cnt[tile] = tot;
+  }
+}
+
+// One CTA per segment: tie_off[tile] = ties of the segment in the tiles before this one.
+__global__ void __launch_bounds__(kSweepThreads) k_rigl_tie_scan(const Seg* __restrict__ segs, const RiglSel* __restrict__ sel,
+                                                                 const unsigned int* __restrict__ tie_cnt,
+                                                                 unsigned int* __restrict__ tie_off) {
+  __shared__ unsigned int s_red[kSweepThreads / 32];
+  if (sel[blockIdx.x].none) return;
+  const Seg sg = segs[blockIdx.x];
+  const long long nt = (sg.n + kTileElems - 1) / kTileElems;
+  unsigned int carry = 0;
+  for (long long c0 = 0; c0 < nt; c0 += kSweepThreads) {
+    const long long i = c0 + threadIdx.x;
+    const unsigned int v = i < nt ? tie_cnt[sg.tile0 + i] : 0u;
+    unsigned int tot;
+    const unsigned int ex = block_excl_scan_u32(v, s_red, &tot);
+    if (i < nt) tie_off[sg.tile0 + i] = carry + ex;
+    carry += tot;
+  }
+}
+
+template <int PHASE>
+__global__ void __launch_bounds__(kSweepThreads) k_rigl_write(const Seg* __restrict__ segs, int n_seg, long long tiles,
+                                                              const RiglSel* __restrict__ sel,
+                                                              const unsigned int* __restrict__ tie_cnt,
+                                                              const unsigned int* __restrict__ tie_off,
+                                                              unsigned long long* __restrict__ counts) {
+  __shared__ unsigned int s_red[kSweepThreads / 32];
+  const int t = threadIdx.x;
+  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int si = find_seg(segs, n_seg, tile);
+    const RiglSel s = sel[si];
+    if (PHASE == 1 && s.none) continue;               // GROW leaves such a segment as the DROP wrote it
+    const Seg sg = segs[si];
+    const long long base = (tile - sg.tile0) * kTileElems;
+    const long long rem = sg.n - base;
+    const int n_in = rem < kTileElems ? (int)rem : kTileElems;
+    unsigned int key[kRiglPer];
+    const unsigned int elig = rigl_load<PHASE>(sg, base, n_in, key);
+    unsigned int picked = 0;
+    if (!s.none) {
+      const unsigned int T = s.prefix;
+      unsigned int ord = 0;
+      if (tie_cnt[tile]) {                              // this tile holds ties at T: their rank in the segment
+        unsigned int mine = 0, tot;
+#pragma unroll
+        for (int j = 0; j < kRiglPer; ++j) mine += ((elig >> j) & 1u) && key[j] == T;
+        ord = tie_off[tile] + block_excl_scan_u32(mine, s_red, &tot);
+      }
+#pragma unroll
+      for (int j = 0; j < kRiglPer; ++j) {
+        if (!((elig >> j) & 1u)) continue;
+        if (key[j] < T) picked |= 1u << j;
+        else if (key[j] == T) { if ((unsigned long long)ord < s.k_rem) picked |= 1u << j; ++ord; }
+      }
+    }
+    const int j0 = t * kRiglPer;
+    float* o = sg.mo + base + j0;
+    if (PHASE == 0) {
+      const unsigned int keep = elig & ~picked;
+      if (n_in - j0 >= kRiglPer && (((uintptr_t)o) & 15) == 0) {
+#pragma unroll
+        for (int q = 0; q < kRiglPer / 4; ++q)
+          ((float4*)o)[q] = make_float4((float)((keep >> (4 * q)) & 1u), (float)((keep >> (4 * q + 1)) & 1u),
+                                        (float)((keep >> (4 * q + 2)) & 1u), (float)((keep >> (4 * q + 3)) & 1u));
+      } else {
+        for (int j = 0; j < kRiglPer && j0 + j < n_in; ++j) o[j] = (float)((keep >> j) & 1u);
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < kRiglPer; ++j)
+        if ((picked >> j) & 1u) o[j] = 1.f;
+    }
+    const unsigned int tot = block_sum_u32(__popc(picked), s_red);
+    if (t == 0 && tot) atomicAdd(&counts[2 * si + PHASE], (unsigned long long)tot);
+  }
+}
+
+// mask <- new; where new != 0 and old == 0 the weight and its momentum (if any) restart from 0.
+// Seg: m = mask (written), g = new mask, w = weight (written), buf = momentum (nullable).
+__global__ void __launch_bounds__(kSweepThreads) k_rigl_apply(const Seg* __restrict__ segs, int n_seg, long long tiles) {
+  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int si = find_seg(segs, n_seg, tile);
+    const Seg sg = segs[si];
+    const long long base = (tile - sg.tile0) * kTileElems;
+    const long long rem = sg.n - base;
+    const int n_in = rem < kTileElems ? (int)rem : kTileElems;
+    float* m = const_cast<float*>(sg.m) + base;
+    float* w = const_cast<float*>(sg.w) + base;
+    float* buf = sg.buf ? sg.buf + base : nullptr;
+    const float* nm = sg.g + base;
+    for (int i = threadIdx.x; i < n_in; i += kSweepThreads) {
+      const float old = m[i], nw = nm[i];
+      if (nw != 0.f && old == 0.f) { w[i] = 0.f; if (buf) buf[i] = 0.f; }
+      if (__float_as_uint(nw) != __float_as_uint(old)) m[i] = nw;
+    }
+  }
+}
+
+struct RiglWs {
+  Seg* segs; RiglSel* sel; unsigned int* hist; unsigned int* tie_cnt; unsigned int* tie_off;
+};
+
+static long long rigl_max_tiles(int n_seg, long long total) { return total / kTileElems + n_seg + 1; }
+
+template <int PHASE>
+static int rigl_phase(const RiglWs& w, int n_seg, long long tiles, unsigned long long* counts, cudaStream_t st) {
+  const int grid = sweep_grid(tiles);
+  RiglSel* sel = w.sel + (size_t)PHASE * n_seg;
+  const int shifts[3] = {21, 10, 0}, bits[3] = {11, 11, 10};
+  for (int p = 0; p < 3; ++p) {
+    k_rigl_hist<PHASE><<<grid, kSweepThreads, 0, st>>>(w.segs, n_seg, tiles, sel, shifts[p], bits[p], w.hist);
+    k_rigl_pick<<<n_seg, kSweepThreads, 0, st>>>(w.hist, sel, PHASE == 1 ? w.sel : nullptr, shifts[p], bits[p], p == 0);
+  }
+  k_rigl_ties<PHASE><<<grid, kSweepThreads, 0, st>>>(w.segs, n_seg, tiles, sel, w.tie_cnt);
+  k_rigl_tie_scan<<<n_seg, kSweepThreads, 0, st>>>(w.segs, sel, w.tie_cnt, w.tie_off);
+  k_rigl_write<PHASE><<<grid, kSweepThreads, 0, st>>>(w.segs, n_seg, tiles, sel, w.tie_cnt, w.tie_off, counts);
+  TP_LAUNCH_CHECK();
+  return TP_OK;
+}
+
 }  // namespace tp
 
 using namespace tp;
@@ -788,6 +1094,67 @@ int tp_count_zeros(const void* const* m, const int64_t* numel, int n_seg,
   TP_CUDA_CHECK(cudaMemsetAsync(zeros_out, 0, sizeof(int64_t) * (size_t)(n_seg + 1), st));
   if (tiles == 0) return TP_OK;
   k_count_zeros<<<sweep_grid(tiles), kSweepThreads, 0, st>>>(d_segs, n_seg, tiles, (unsigned long long*)zeros_out);
+  TP_LAUNCH_CHECK();
+  return TP_OK;
+}
+
+size_t tp_rigl_workspace_bytes(int n_seg, int64_t total_numel) {
+  const size_t ns = (size_t)(n_seg > 0 ? n_seg : 1);
+  const size_t tiles = (size_t)rigl_max_tiles((int)ns, total_numel);
+  return align_up(sizeof(Seg) * ns, 256) + align_up(sizeof(RiglSel) * 2 * ns, 256) + align_up(sizeof(unsigned int) * 2048 * ns, 256) +
+         2 * align_up(sizeof(unsigned int) * tiles, 256) + 1024;
+}
+
+int tp_rigl_select(const void* const* w, const void* const* g, const void* const* mask, void* const* new_mask_out,
+                   const int64_t* numel, const int64_t* k, int n_seg, int64_t* counts_out, void* ws, size_t ws_bytes,
+                   void* stream) {
+  if (!w || !g || !mask || !new_mask_out || !numel || !k || n_seg <= 0 || !counts_out || !ws) return TP_ERR_INVALID;
+  for (int i = 0; i < n_seg; ++i) {
+    if (!w[i] || !g[i] || !mask[i] || !new_mask_out[i]) return TP_ERR_INVALID;
+    if (numel[i] < 0 || numel[i] > (1ll << 31) || k[i] < 0) return TP_ERR_INVALID;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  Arena ar(ws, ws_bytes);
+  RiglWs t;
+  long long tiles = 0, total = 0;
+  int rc = upload_segs(ar, w, g, mask, new_mask_out, nullptr, numel, n_seg, &t.segs, &tiles, &total, st);
+  if (rc) return rc;
+  t.sel = (RiglSel*)ar.take(sizeof(RiglSel) * 2 * (size_t)n_seg);
+  t.hist = (unsigned int*)ar.take(sizeof(unsigned int) * 2048 * (size_t)n_seg);
+  t.tie_cnt = (unsigned int*)ar.take(sizeof(unsigned int) * (size_t)(tiles > 0 ? tiles : 1));
+  t.tie_off = (unsigned int*)ar.take(sizeof(unsigned int) * (size_t)(tiles > 0 ? tiles : 1));
+  if (!t.sel || !t.hist || !t.tie_cnt || !t.tie_off) return TP_ERR_WORKSPACE;
+  std::vector<RiglSel> h(2 * (size_t)n_seg);
+  for (int p = 0; p < 2; ++p)
+    for (int i = 0; i < n_seg; ++i) {
+      RiglSel& s = h[(size_t)p * n_seg + i];
+      s = RiglSel{};
+      s.k = (unsigned long long)k[i];
+      s.k_rem = s.k;
+      s.none = k[i] == 0;
+    }
+  // pageable source: the runtime stages the bytes before returning, so `h` may die.
+  TP_CUDA_CHECK(cudaMemcpyAsync(t.sel, h.data(), sizeof(RiglSel) * h.size(), cudaMemcpyHostToDevice, st));
+  TP_CUDA_CHECK(cudaMemsetAsync(t.hist, 0, sizeof(unsigned int) * 2048 * (size_t)n_seg, st));   // the picks clear it after use
+  TP_CUDA_CHECK(cudaMemsetAsync(counts_out, 0, sizeof(int64_t) * 2 * (size_t)n_seg, st));
+  if (tiles == 0) return TP_OK;
+  rc = rigl_phase<0>(t, n_seg, tiles, (unsigned long long*)counts_out, st); if (rc) return rc;
+  return rigl_phase<1>(t, n_seg, tiles, (unsigned long long*)counts_out, st);
+}
+
+int tp_rigl_apply(void* const* mask, const void* const* new_mask, void* const* w, void* const* momentum,
+                  const int64_t* numel, int n_seg, void* ws, size_t ws_bytes, void* stream) {
+  if (!mask || !new_mask || !w || !numel || n_seg <= 0 || !ws) return TP_ERR_INVALID;
+  for (int i = 0; i < n_seg; ++i)
+    if (!mask[i] || !new_mask[i] || !w[i] || numel[i] < 0 || numel[i] > (1ll << 31)) return TP_ERR_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  Arena ar(ws, ws_bytes);
+  Seg* d_segs = nullptr; long long tiles = 0;
+  int rc = upload_segs(ar, (const void* const*)w, new_mask, (const void* const*)mask, nullptr, momentum, numel, n_seg,
+                       &d_segs, &tiles, nullptr, st);
+  if (rc) return rc;
+  if (tiles == 0) return TP_OK;
+  k_rigl_apply<<<sweep_grid(tiles), kSweepThreads, 0, st>>>(d_segs, n_seg, tiles);
   TP_LAUNCH_CHECK();
   return TP_OK;
 }

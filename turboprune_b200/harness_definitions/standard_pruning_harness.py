@@ -8,6 +8,11 @@ reference's device-resident CIFAR loader (``AirbenchLoaders``) when a CIFAR conf
 other than ``synthetic`` (the reference's ``dp_cifar*.yaml`` say ``torch``); ``ImageFolderImagenet`` (GPU-decoded
 ImageFolder tree) when an ImageNet config says ``dataloader_type: imagefolder``; otherwise (FFCV / WebDataset are out of
 scope) the synthetic on-device generator.
+
+``pruning_params.training_type: rigl`` trains with dynamic sparse masks (RigL, utils/rigl.py): on an update batch the
+harness runs one eager forward / backward with dense weight gradients instead of the train step, drops and regrows
+weights in place (``pruning_utils.rigl_update``), takes no optimizer step and zeroes the gradients.  Every other batch
+is the ordinary train step, whose captured CUDA graph stays valid across updates.
 """
 import csv
 import os
@@ -16,12 +21,14 @@ from typing import Optional
 
 import torch
 import torch.nn as nn
+from torch.amp import autocast
 
 from ..optim import FusedSGD
 from ..utils import schedulers
 from ..utils.custom_models import CustomModel, TorchVisionModel
 from ..utils.dataset import AirbenchLoaders, ImageFolderImagenet, SyntheticLoaders
 from ..utils.harness_utils import save_model
+from ..utils.rigl import RiglSchedule, rigl_params
 from .base_harness import BaseHarness
 
 
@@ -36,6 +43,8 @@ class PruningHarness(BaseHarness):
         self.prefix, self.expt_dir = expt_dir
         distributed = (cfg.experiment_params.distributed and torch.distributed.is_available()
                        and torch.distributed.is_initialized() and not self.dataset_name.startswith("cifar"))
+        self._rigl_params = rigl_params(cfg)          # raises ValueError for a config RigL cannot start from
+        self.rigl = None                               # this level's RiglSchedule (train_one_level / begin_rigl_level)
         super().__init__(cfg=cfg, device=self.this_device, model=model, distributed=distributed)
 
     def _create_model(self):
@@ -86,6 +95,8 @@ class PruningHarness(BaseHarness):
         model = self.model
         self._setup_optimizer()
         self._setup_scheduler(epochs_per_level)
+        if self._rigl_params is not None:
+            self.begin_rigl_level(epochs_per_level)
         ck = os.path.join(self.expt_dir, "checkpoints")
         art = os.path.join(self.expt_dir, "artifacts")
         if self.gpu_id == 0 and level == 0:
@@ -115,3 +126,60 @@ class PruningHarness(BaseHarness):
                 if new:
                     w.writerow(["Level", "Sparsity", "Last_Test_Acc", "Max_Test_Acc"])
                 w.writerow([level, model.get_overall_sparsity(), rows[-1]["test_acc"], max(r["test_acc"] for r in rows)])
+
+    # ---- RigL: dynamic sparse masks within a level ---------------------------------------------------------------
+    def _masked_layers(self):
+        from ..utils.mask_layers import MASKED_LAYER_TYPES
+        return [m for m in self.model.modules() if isinstance(m, MASKED_LAYER_TYPES)]
+
+    def begin_rigl_level(self, epochs_per_level: int) -> None:
+        """Start a RigL level of ``epochs_per_level * len(train_loader)`` batches: count every layer's active weights
+        (one host sync; RigL keeps the counts) and allocate the scratch masks the updates reuse."""
+        from .. import ops
+        layers = self._masked_layers()
+        for m in layers:
+            if m.mask.device != m.weight.device or m.mask.dtype != torch.float32 or not m.mask.is_contiguous():
+                m.mask = m.mask.to(device=m.weight.device, dtype=torch.float32).contiguous()
+        zeros = ops.count_zeros([m.mask for m in layers]).cpu().tolist()
+        self.rigl = RiglSchedule(*self._rigl_params, total_steps=epochs_per_level * len(self.train_loader))
+        self.rigl_active = [m.mask.numel() - z for m, z in zip(layers, zeros)]
+        self.rigl_step = 0                         # batches consumed in this level
+        self.rigl_counts = None                    # (dropped, grown) per layer of the last update, int64 cuda [layers, 2]
+        self._rigl_new = [torch.empty_like(m.mask) for m in layers]
+
+    def train_step(self, batch):
+        t = getattr(self, "rigl_step", None)
+        if self.rigl is not None and self.rigl.is_update(t):
+            out = self._rigl_update_step(batch, self.rigl.k_per_layer(t, self.rigl_active))
+        else:
+            out = super().train_step(batch)
+        if self.rigl is not None:
+            self.rigl_step = t + 1
+        return out
+
+    def _rigl_update_step(self, batch, k_per_layer):
+        """Dense-gradient forward / backward, drop-and-regrow in place, no optimizer step.  Under torch.distributed
+        every rank uses its own dense gradient (no exchange on this batch) and rank 0's masks are imposed."""
+        from .. import fused_norm, ops
+        from ..utils.pruning_utils import rigl_update
+        inputs, targets = batch
+        inputs, targets = inputs.to(self.device, non_blocking=True), targets.to(self.device, non_blocking=True)
+        store = self._grad_store()
+        store.zero()
+        with self._compute_precision(), ops.dense_weight_grad():
+            self._weight_stager().stage()
+            with autocast(device_type="cuda", dtype=self.precision, enabled=self.use_amp):
+                outputs = self.model(inputs)
+                loss = self.criterion(outputs, targets)
+            try:
+                loss.backward()
+            finally:
+                ops.join_wgrad(self.device)
+                fused_norm.drop_partials()
+        self.rigl_counts = rigl_update(self.model, self.optimizer, k_per_layer, new_masks=self._rigl_new)
+        if self.reducer is not None:
+            self.reducer.set_model_masks(getattr(self.model, "model", self.model))     # in place: same buffers
+        store.zero()
+        self._drop_staged()                        # the next step restages the weights from the new masks
+        self.train_accuracy.update(outputs.detach(), targets)
+        return {"loss": loss.detach()}

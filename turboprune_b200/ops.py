@@ -42,6 +42,40 @@ def compute_precision(dtype):
             _precision.dtype = prev
 
 
+# ---- dense weight gradients --------------------------------------------------------------------------------------------
+# Inside ``dense_weight_grad()`` the masked layers write the UNMASKED weight gradient wgrad(x, dy) (RigL's grow
+# criterion needs |g| at pruned positions).  The forward is unchanged.  Read in the forward and kept in ctx, like the
+# precision.
+_dense_grad = threading.local()
+
+
+def dense_grad_enabled():
+    return getattr(_dense_grad, "on", False)
+
+
+@contextmanager
+def dense_weight_grad(on=True):
+    """Masked layers whose forward runs inside this block produce the dense weight gradient in their backward."""
+    prev = dense_grad_enabled()
+    _dense_grad.on = bool(on)
+    try:
+        yield
+    finally:
+        _dense_grad.on = prev
+
+
+_ones_cache = {}
+
+
+def _ones_like_mask(m):
+    """Cached all-ones fp32 mask of m's shape (the wgrad kernels take a mask; a dense gradient hands them this one)."""
+    key = (tuple(m.shape), m.device)
+    t = _ones_cache.get(key)
+    if t is None:
+        t = _ones_cache[key] = torch.ones(m.shape, dtype=torch.float32, device=m.device)
+    return t
+
+
 def _count(n=1):
     global _launches
     _launches += n
@@ -318,6 +352,50 @@ def count_zeros(ms):
     _cabi.check(rc, "tp_count_zeros")
     _count()
     return out
+
+
+def rigl_select(ws, gs, ms, new_ms, ks):
+    """RigL drop-and-regrow selection for all layers in one launch sequence (no host sync): writes the mask after the
+    update into ``new_ms`` (``ms`` is not written).  Per layer i: drop the ks[i] smallest |w| among ms[i] != 0, then grow
+    the ks[i] largest |g| among the positions that are 0 after the drop; ties in flat-index order.  Returns an int64
+    cuda tensor [n, 2] of (dropped, grown) counts."""
+    lib = _cabi.load()
+    _require_cuda(*ws, *gs, *ms, *new_ms)
+    for t in list(ws) + list(gs) + list(ms) + list(new_ms):
+        if t.dtype != torch.float32 or not t.is_contiguous():
+            raise TypeError("rigl_select: contiguous fp32 weights / gradients / masks")
+    dev = ws[0].device
+    numel = [w.numel() for w in ws]
+    if any(t.numel() != n for n, g, m, o in zip(numel, gs, ms, new_ms) for t in (g, m, o)):
+        raise ValueError("rigl_select: weight, gradient and mask sizes differ")
+    counts = torch.empty(len(ws), 2, dtype=torch.int64, device=dev)
+    wsb = _workspace(lib.tp_rigl_workspace_bytes(len(ws), sum(numel)), dev, "rigl")
+    with torch.cuda.device(dev):
+        rc = lib.tp_rigl_select(_cabi.ptr_array(ws), _cabi.ptr_array(gs), _cabi.ptr_array(ms), _cabi.ptr_array(new_ms),
+                                _cabi.i64_array(numel), _cabi.i64_array(ks), len(ws), c_void_p(counts.data_ptr()),
+                                c_void_p(wsb.data_ptr()), wsb.numel(), _cabi.stream_ptr(dev))
+    _cabi.check(rc, "tp_rigl_select")
+    _count(20)
+    return counts
+
+
+def rigl_apply(ms, new_ms, ws, bufs=None):
+    """In place, one launch: ms <- new_ms; where new != 0 and old == 0, w = 0 and its momentum (``bufs[i]``, may be
+    None) = 0."""
+    lib = _cabi.load()
+    _require_cuda(*ms, *new_ms, *ws)
+    bufs = [None] * len(ms) if bufs is None else list(bufs)
+    for t in list(ms) + list(new_ms) + list(ws) + [b for b in bufs if b is not None]:
+        if t.dtype != torch.float32 or not t.is_contiguous():
+            raise TypeError("rigl_apply: contiguous fp32 masks / weights / momenta")
+    dev = ms[0].device
+    wsb = _workspace(lib.tp_segtable_workspace_bytes(len(ms)), dev, "seg")
+    with torch.cuda.device(dev):
+        rc = lib.tp_rigl_apply(_cabi.ptr_array(ms), _cabi.ptr_array(new_ms), _cabi.ptr_array(ws), _cabi.ptr_array(bufs),
+                               _cabi.i64_array([m.numel() for m in ms]), len(ms), c_void_p(wsb.data_ptr()), wsb.numel(),
+                               _cabi.stream_ptr(dev))
+    _cabi.check(rc, "tp_rigl_apply")
+    _count()
 
 
 # ---------------------------------------------------------------------------------------------
@@ -919,9 +997,13 @@ def _fp32_backward(ctx, dy):
             ones = torch.ones(cout, kp, dtype=torch.float32, device=xg.device)
             dwm = conv_wgrad_f32(gd, xs, dys, ones.view(cout, kp, 1, 1), kp)
             cg = stem_geometry(cin, r, s)[0]
-            dw = dwm[:, :r * s * cg].reshape(cout, r * s, cg)[:, :, :cin].permute(0, 2, 1).reshape(cout, cin, r, s) * m32
+            dw = dwm[:, :r * s * cg].reshape(cout, r * s, cg)[:, :, :cin].permute(0, 2, 1).reshape(cout, cin, r, s)
+            if not ctx.dense:
+                dw = dw * m32
     else:
         xn, m32, wd = ctx.saved_tensors
+        if ctx.dense:
+            m32 = _ones_like_mask(m32)
         cin = ctx.cin
         ddesc = desc
         if ctx.cout_p != cout:
@@ -977,6 +1059,7 @@ class MaskedConv2dFn(torch.autograd.Function):
     def forward(ctx, x, weight, mask, bias, stride, padding, want_skip=False, grad_slots=None, staged=None, want_stats=False,
                 bn_src=None):
         _require_cuda(x, weight, mask)
+        ctx.dense = dense_grad_enabled()                  # read once, like the precision: dW = wgrad(x, dy), unmasked
         if current_precision() == torch.float32:        # read once; backward follows ctx.f32
             return _fp32_forward(ctx, x, weight, mask, bias, stride, padding, want_skip, grad_slots, staged, want_stats)
         ctx.set_materialize_grads(False)
@@ -1080,9 +1163,14 @@ class MaskedConv2dFn(torch.autograd.Function):
                 dwm, db = conv_wgrad(gd, xg, dyn.view(-1, cout), ones.view(cout, -1, 1, 1), xg.shape[1], need_db)
                 # columns are (tap, channel group): back to OIHW and apply the mask (9.4 k elements)
                 cg = stem_geometry(cin, r, s)[0]
-                dw = dwm[:, :r * s * cg].reshape(cout, r * s, cg)[:, :, :cin].permute(0, 2, 1).reshape(cout, cin, r, s) * m32
+                dw = dwm[:, :r * s * cg].reshape(cout, r * s, cg)[:, :, :cin].permute(0, 2, 1).reshape(cout, cin, r, s)
+                if not ctx.dense:
+                    dw = dw * m32
         else:
             xn, m32, wd = ctx.saved_tensors
+            wf_kmask = ctx.wf_kmask
+            if ctx.dense:                      # all-ones mask and no occupancy mask: every tile of dW is computed
+                m32, wf_kmask = _ones_like_mask(m32), None
             cin = ctx.cin                      # real input channels (desc.cin is the padded count the activation carries)
             ddesc = desc
             if ctx.cout_p != cout:
@@ -1127,14 +1215,14 @@ class MaskedConv2dFn(torch.autograd.Function):
                         side.wait_event(ev)
                         with torch.cuda.stream(side):
                             conv_wgrad(desc, xn, dyn, m32, cin, need_db, dw_out=ws_, db_out=bs_ if direct_b else None,
-                                       kmask=ctx.wf_kmask)
+                                       kmask=wf_kmask)
                             grad_ready(ws_, bs_ if direct_b else None)
                         _wgrad_keepalive.append((xn, dyn, m32))
                         dw = db = None
                         db_in_slot = direct_b
                     else:
                         dw, db = conv_wgrad(desc, xn, dyn, m32, cin, need_db, dw_out=ws_ if direct_w else None,
-                                            db_out=bs_ if direct_b else None, kmask=ctx.wf_kmask)
+                                            db_out=bs_ if direct_b else None, kmask=wf_kmask)
                         if direct_w:
                             dw = None
                         if direct_b:

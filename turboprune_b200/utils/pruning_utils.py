@@ -204,6 +204,53 @@ def sync_masks_from_rank0(model: nn.Module) -> None:
         off += n
 
 
+def sync_masks_from_rank0_(masks) -> None:
+    """In-place form of ``sync_masks_from_rank0``: rank 0's values are broadcast INTO the given tensors (one packed
+    broadcast), so every pointer a captured CUDA graph or a cached table holds stays valid."""
+    import torch.distributed as dist
+    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size() == 1:
+        return
+    masks = list(masks)
+    flat = torch.cat([m.reshape(-1) for m in masks])
+    dist.broadcast(flat, 0)
+    off = 0
+    for m in masks:
+        n = m.numel()
+        m.copy_(flat[off:off + n].view_as(m))
+        off += n
+
+
+@torch.no_grad()
+def rigl_update(model: nn.Module, optimizer, k_per_layer, new_masks=None):
+    """One RigL drop-and-regrow step (Evci et al. 2020) over the masked layers' current ``.grad``.
+
+    The gradients must be dense: run the forward / backward inside ``ops.dense_weight_grad()``.  Per masked layer l,
+    the k_per_layer[l] live weights of smallest |w| are dropped and as many pruned positions of largest |g| (the
+    just-dropped ones included) are grown; ties go to the lower flat index.  Grown weights and their momentum
+    (``optimizer.state[w]['momentum_buffer']`` when there is one) restart at 0; regrown dropped weights keep theirs.
+    Masks, weights and momenta are updated in place (``mask_layers.mask_epoch()`` does not change).  Under
+    torch.distributed every rank selects, rank 0's result is broadcast, every rank applies it.  ``new_masks``:
+    scratch tensors of the masks' shapes to reuse.  Returns an int64 cuda tensor [layers, 2] of (dropped, grown)."""
+    layers = _masked(model)
+    for m in layers:
+        if m.weight.grad is None:
+            raise RuntimeError("rigl_update: a masked layer has no gradient (run a backward pass inside "
+                               "ops.dense_weight_grad() first)")
+        if m.mask.device != m.weight.device or m.mask.dtype != torch.float32 or not m.mask.is_contiguous():
+            m.mask = m.mask.to(device=m.weight.device, dtype=torch.float32).contiguous()
+    ws = [m.weight.detach() for m in layers]
+    gs = [m.weight.grad.contiguous() for m in layers]
+    ms = [m.mask for m in layers]
+    if new_masks is None:
+        new_masks = [torch.empty_like(m) for m in ms]
+    counts = ops.rigl_select(ws, gs, ms, new_masks, k_per_layer)
+    sync_masks_from_rank0_(new_masks)
+    state = getattr(optimizer, "state", {}) if optimizer is not None else {}
+    bufs = [state[m.weight].get("momentum_buffer") if m.weight in state else None for m in layers]
+    ops.rigl_apply(ms, new_masks, ws, bufs)
+    return counts
+
+
 def prune_the_model(cfg, harness, target_density: float) -> None:
     """Dispatcher by ``cfg.pruning_params.prune_method`` (reference :23-58)."""
     # the reference unwraps DDP here (:25); our harness keeps the bare module and reduces gradients explicitly
