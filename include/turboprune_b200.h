@@ -115,6 +115,13 @@ int tp_rigl_select(const void* const* w, const void* const* g, const void* const
  * or the whole array may be NULL).  One launch.  Workspace: tp_segtable_workspace_bytes(n_seg). */
 int tp_rigl_apply(void* const* mask, const void* const* new_mask, void* const* w, void* const* momentum,
                   const int64_t* numel, int n_seg, void* ws, size_t ws_bytes, void* stream);
+/* The same apply for any number of per-element optimizer state arrays (SGD: momentum_buffer; AdamW: exp_avg and
+ * exp_avg_sq): where new_mask != 0 and mask == 0 the weight and every state restart from 0.  states: HOST array of
+ * n_states * n_seg DEVICE pointers, states[j * n_seg + i] = state j of segment i (entries may be NULL; states may be
+ * NULL when n_states == 0).  tp_rigl_apply is the n_states = 1 call.  One launch.
+ * Workspace: tp_segtable_workspace_bytes(n_seg * max(n_states, 1)). */
+int tp_rigl_apply_states(void* const* mask, const void* const* new_mask, void* const* w, void* const* states, int n_states,
+                         const int64_t* numel, int n_seg, void* ws, size_t ws_bytes, void* stream);
 
 /* ---- weight staging: fp32 (mask*w) -> bf16 tensor-core operand layouts ------------------
  * Replaces the per-forward `mask * weight` (utils/mask_layers.py:25,69,109) and the autocast
@@ -351,6 +358,22 @@ int tp_sgd_momentum(void* const* w, const void* const* g, void* const* buf, cons
                     int n_seg, const float* lr_dev, float momentum, float weight_decay,
                     int first_step, int table_cached, void* ws, size_t ws_bytes, void* stream);
 size_t tp_segtable_workspace_bytes(int n_seg);
+/* torch.optim.AdamW (decoupled weight decay), bit for bit with its capturable foreach branch, for an optimizer_name:
+ * AdamW config (the reference's harness builds SGD whatever the name says, standard_pruning_harness.py:52-75).  Per
+ * segment, with t its step count after the increment:
+ *   step += 1;  w *= c (decay_dev != NULL);  m = lerp(m, g, 1 - b1);  v = b2 v + (1 - b2) g g;
+ *   s = 1 / ((b1^t - 1) * inv_lr);  b = sqrt(1 - b2^t);  w += m / ((sqrt(v) / b + eps) / s)
+ *   w, g, exp_avg, exp_avg_sq : HOST arrays of n_seg DEVICE pointers (fp32, contiguous)
+ *   step                      : HOST array of n_seg DEVICE pointers to each segment's fp32 step count (0-dim)
+ *   inv_lr_dev                : DEVICE float inv_lr = fp32(1 / lr) computed in double (ATen divides a tensor by a Python
+ *                               scalar this way); decay_dev: DEVICE float c = fp32(1 - lr * weight_decay) computed in
+ *                               double, or NULL when weight_decay == 0.  Neither is baked into a captured graph.
+ *   beta1, beta2, eps         : as the Python floats; 1 - beta is formed in double, then rounded to fp32
+ * Two launches (the step increment, then the update).  table_cached: as tp_sgd_momentum (capturable).
+ * Workspace: tp_segtable_workspace_bytes(n_seg). */
+int tp_adamw(void* const* w, const void* const* g, void* const* exp_avg, void* const* exp_avg_sq, void* const* step,
+             const int64_t* numel, int n_seg, const float* inv_lr_dev, const float* decay_dev,
+             double beta1, double beta2, double eps, int table_cached, void* ws, size_t ws_bytes, void* stream);
 
 /* ---- gradient exchange over NVLink/NVSwitch peer memory ---------------------------------
  * Replaces the c10d Reducer's per-bucket  grad/W -> ncclAllReduce(SUM) -> copy back

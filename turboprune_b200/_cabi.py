@@ -6,7 +6,7 @@ the wrappers raise.
 """
 import ctypes
 import os
-from ctypes import POINTER, c_char_p, c_float, c_int, c_int32, c_int64, c_size_t, c_uint64, c_void_p
+from ctypes import POINTER, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_size_t, c_uint64, c_void_p
 
 from . import build as _build
 
@@ -82,6 +82,11 @@ SIGNATURES = {
     "tp_sgd_momentum": (c_int, [POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_int64), c_int,
                                 c_void_p, c_float, c_float, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "tp_segtable_workspace_bytes": (c_size_t, [c_int]),
+    "tp_adamw": (c_int, [POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p),
+                         POINTER(c_int64), c_int, c_void_p, c_void_p, c_double, c_double, c_double, c_int, c_void_p,
+                         c_size_t, c_void_p]),
+    "tp_rigl_apply_states": (c_int, [POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), c_int,
+                                     POINTER(c_int64), c_int, c_void_p, c_size_t, c_void_p]),
     "tp_p2p_allreduce_mask": (c_int, [POINTER(c_void_p), POINTER(c_void_p), c_int, c_int, c_int64, c_void_p, c_float,
                                       c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "tp_bn_workspace_bytes": (c_size_t, [c_int64, c_int]),

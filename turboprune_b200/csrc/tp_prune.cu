@@ -950,9 +950,11 @@ __global__ void __launch_bounds__(kSweepThreads) k_rigl_write(const Seg* __restr
   }
 }
 
-// mask <- new; where new != 0 and old == 0 the weight and its momentum (if any) restart from 0.
-// Seg: m = mask (written), g = new mask, w = weight (written), buf = momentum (nullable).
-__global__ void __launch_bounds__(kSweepThreads) k_rigl_apply(const Seg* __restrict__ segs, int n_seg, long long tiles) {
+// mask <- new; where new != 0 and old == 0 the weight and its optimizer state (if any) restart from 0.
+// Seg: m = mask (written), g = new mask, w = weight (written), buf = first state array (nullable).
+// xs: the further state arrays, xs[j * n_seg + i] = state j + 1 of segment i (nullable entries), n_xs of them per segment.
+__global__ void __launch_bounds__(kSweepThreads) k_rigl_apply(const Seg* __restrict__ segs, int n_seg, long long tiles,
+                                                              float* const* __restrict__ xs, int n_xs) {
   for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
     const int si = find_seg(segs, n_seg, tile);
     const Seg sg = segs[si];
@@ -965,7 +967,14 @@ __global__ void __launch_bounds__(kSweepThreads) k_rigl_apply(const Seg* __restr
     const float* nm = sg.g + base;
     for (int i = threadIdx.x; i < n_in; i += kSweepThreads) {
       const float old = m[i], nw = nm[i];
-      if (nw != 0.f && old == 0.f) { w[i] = 0.f; if (buf) buf[i] = 0.f; }
+      if (nw != 0.f && old == 0.f) {
+        w[i] = 0.f;
+        if (buf) buf[i] = 0.f;
+        for (int j = 0; j < n_xs; ++j) {
+          float* x = xs[(size_t)j * n_seg + si];
+          if (x) x[base + i] = 0.f;
+        }
+      }
       if (__float_as_uint(nw) != __float_as_uint(old)) m[i] = nw;
     }
   }
@@ -1142,21 +1151,35 @@ int tp_rigl_select(const void* const* w, const void* const* g, const void* const
   return rigl_phase<1>(t, n_seg, tiles, (unsigned long long*)counts_out, st);
 }
 
-int tp_rigl_apply(void* const* mask, const void* const* new_mask, void* const* w, void* const* momentum,
-                  const int64_t* numel, int n_seg, void* ws, size_t ws_bytes, void* stream) {
-  if (!mask || !new_mask || !w || !numel || n_seg <= 0 || !ws) return TP_ERR_INVALID;
+int tp_rigl_apply_states(void* const* mask, const void* const* new_mask, void* const* w, void* const* states, int n_states,
+                         const int64_t* numel, int n_seg, void* ws, size_t ws_bytes, void* stream) {
+  if (!mask || !new_mask || !w || !numel || n_seg <= 0 || !ws || n_states < 0 || (n_states > 0 && !states)) return TP_ERR_INVALID;
   for (int i = 0; i < n_seg; ++i)
     if (!mask[i] || !new_mask[i] || !w[i] || numel[i] < 0 || numel[i] > (1ll << 31)) return TP_ERR_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
   Arena ar(ws, ws_bytes);
   Seg* d_segs = nullptr; long long tiles = 0;
-  int rc = upload_segs(ar, (const void* const*)w, new_mask, (const void* const*)mask, nullptr, momentum, numel, n_seg,
-                       &d_segs, &tiles, nullptr, st);
+  int rc = upload_segs(ar, (const void* const*)w, new_mask, (const void* const*)mask, nullptr, n_states > 0 ? states : nullptr,
+                       numel, n_seg, &d_segs, &tiles, nullptr, st);
   if (rc) return rc;
+  // states past the first: a pointer array behind the segment table
+  const int n_xs = n_states > 1 ? n_states - 1 : 0;
+  float** d_xs = nullptr;
+  if (n_xs > 0) {
+    d_xs = (float**)ar.take(sizeof(float*) * (size_t)n_xs * n_seg);
+    if (!d_xs) return TP_ERR_WORKSPACE;
+    // pageable source: the runtime stages the bytes before returning
+    TP_CUDA_CHECK(cudaMemcpyAsync(d_xs, states + n_seg, sizeof(float*) * (size_t)n_xs * n_seg, cudaMemcpyHostToDevice, st));
+  }
   if (tiles == 0) return TP_OK;
-  k_rigl_apply<<<sweep_grid(tiles), kSweepThreads, 0, st>>>(d_segs, n_seg, tiles);
+  k_rigl_apply<<<sweep_grid(tiles), kSweepThreads, 0, st>>>(d_segs, n_seg, tiles, d_xs, n_xs);
   TP_LAUNCH_CHECK();
   return TP_OK;
+}
+
+int tp_rigl_apply(void* const* mask, const void* const* new_mask, void* const* w, void* const* momentum,
+                  const int64_t* numel, int n_seg, void* ws, size_t ws_bytes, void* stream) {
+  return tp_rigl_apply_states(mask, new_mask, w, momentum, momentum ? 1 : 0, numel, n_seg, ws, ws_bytes, stream);
 }
 
 }  // extern "C"

@@ -3,7 +3,8 @@
 ``PruningHarness(cfg, gpu_id, expt_dir, model=None)`` and ``.train_one_level(epochs_per_level, level)`` keep the
 reference's behaviour (:28-50, :159-269): a fresh optimizer and LR schedule per level (momentum never carries
 over), ``model_init.pt`` / ``optimizer_init.pt`` at level 0, ``model_rewind.pt`` at ``pruning_params.rewind_epoch``,
-per-level CSV + summary CSV.  Optimizer = ``FusedSGD`` (same state-dict layout as torch.optim.SGD).  Loaders: the
+per-level CSV + summary CSV.  Optimizer = ``FusedSGD`` (same state-dict layout as torch.optim.SGD), or ``FusedAdamW``
+(torch.optim.AdamW's) when ``optimizer_params.optimizer_name`` is ``AdamW``.  Loaders: the
 reference's device-resident CIFAR loader (``AirbenchLoaders``) when a CIFAR config names a ``dataset_params.dataloader_type``
 other than ``synthetic`` (the reference's ``dp_cifar*.yaml`` say ``torch``); ``ImageFolderImagenet`` (GPU-decoded
 ImageFolder tree) when an ImageNet config says ``dataloader_type: imagefolder``; otherwise (FFCV / WebDataset are out of
@@ -23,7 +24,7 @@ import torch
 import torch.nn as nn
 from torch.amp import autocast
 
-from ..optim import FusedSGD
+from ..optim import FusedAdamW, FusedSGD
 from ..utils import schedulers
 from ..utils.custom_models import CustomModel, TorchVisionModel
 from ..utils.dataset import AirbenchLoaders, ImageFolderImagenet, SyntheticLoaders
@@ -77,6 +78,11 @@ class PruningHarness(BaseHarness):
             raise NotImplementedError("ScheduleFree optimizer (third-party package, off the benchmarked path)")
         # capturable: the learning rate is a device scalar refreshed by train_step (sync_lr), so the captured step
         # follows the per-iteration LR schedule without being re-recorded
+        if o.get("optimizer_name", "SGD") == "AdamW":
+            self.optimizer = FusedAdamW(self.model.parameters(), lr=o.lr, betas=tuple(o.get("betas") or (0.9, 0.999)),
+                                        eps=o.get("eps") or 1e-8, weight_decay=o.weight_decay, capturable=True)
+            return
+        # SGD, and (as in the reference, whose harness builds SGD whatever the name says) every other name
         self.optimizer = FusedSGD(self.model.parameters(), lr=o.lr, momentum=o.momentum, weight_decay=o.weight_decay,
                                   capturable=True)
 

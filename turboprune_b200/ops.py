@@ -398,6 +398,29 @@ def rigl_apply(ms, new_ms, ws, bufs=None):
     _count()
 
 
+def rigl_apply_states(ms, new_ms, ws, states):
+    """``rigl_apply`` for any number of optimizer state arrays: ``states[j][i]`` is state j of layer i (None allowed).
+    Where new != 0 and old == 0, w and every state restart at 0.  One launch."""
+    lib = _cabi.load()
+    _require_cuda(*ms, *new_ms, *ws)
+    states = [list(s) for s in states]
+    if any(len(s) != len(ms) for s in states):
+        raise ValueError("rigl_apply_states: one state tensor (or None) per layer")
+    for t in list(ms) + list(new_ms) + list(ws) + [b for s in states for b in s if b is not None]:
+        if t.dtype != torch.float32 or not t.is_contiguous():
+            raise TypeError("rigl_apply_states: contiguous fp32 masks / weights / optimizer states")
+    dev = ms[0].device
+    wsb = _workspace(lib.tp_segtable_workspace_bytes(len(ms) * max(len(states), 1)), dev, "seg")
+    flat = [b for s in states for b in s]
+    with torch.cuda.device(dev):
+        rc = lib.tp_rigl_apply_states(_cabi.ptr_array(ms), _cabi.ptr_array(new_ms), _cabi.ptr_array(ws),
+                                      _cabi.ptr_array(flat) if flat else None, len(states),
+                                      _cabi.i64_array([m.numel() for m in ms]), len(ms), c_void_p(wsb.data_ptr()),
+                                      wsb.numel(), _cabi.stream_ptr(dev))
+    _cabi.check(rc, "tp_rigl_apply_states")
+    _count()
+
+
 # ---------------------------------------------------------------------------------------------
 # optimizer
 # ---------------------------------------------------------------------------------------------
@@ -414,6 +437,25 @@ def sgd_momentum_step(params, grads, bufs, lr_dev, momentum, weight_decay, first
                                  int(bool(table_cached)), c_void_p(wsb.data_ptr()), wsb.numel(), _cabi.stream_ptr(dev))
     _cabi.check(rc, "tp_sgd_momentum")
     _count()
+
+
+def adamw_step(params, grads, exp_avgs, exp_avg_sqs, steps, inv_lr_dev, decay_dev, beta1, beta2, eps, table_ws=None,
+               table_cached=False):
+    """One fused AdamW step (step-count increment + update: two launches).  ``inv_lr_dev``: device fp32(1 / lr) and
+    ``decay_dev``: device fp32(1 - lr * wd), or None for weight_decay == 0, both formed in double.  ``table_ws`` /
+    ``table_cached``: as ``sgd_momentum_step``."""
+    lib = _cabi.load()
+    dev = params[0].device
+    wsb = table_ws if table_ws is not None else _workspace(lib.tp_segtable_workspace_bytes(len(params)), dev, "seg")
+    # a cached table needs no pointers (the call only counts tiles), which saves the host five pointer arrays per step
+    ptrs = [None] * 5 if table_cached else [_cabi.ptr_array(ts) for ts in (params, grads, exp_avgs, exp_avg_sqs, steps)]
+    with torch.cuda.device(dev):
+        rc = lib.tp_adamw(*ptrs, _cabi.i64_array([p.numel() for p in params]),
+                          len(params), c_void_p(inv_lr_dev.data_ptr()), c_void_p(decay_dev.data_ptr()) if decay_dev is not None else None,
+                          float(beta1), float(beta2), float(eps), int(bool(table_cached)), c_void_p(wsb.data_ptr()),
+                          wsb.numel(), _cabi.stream_ptr(dev))
+    _cabi.check(rc, "tp_adamw")
+    _count(2)
 
 
 # ---------------------------------------------------------------------------------------------

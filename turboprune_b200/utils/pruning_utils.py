@@ -226,8 +226,9 @@ def rigl_update(model: nn.Module, optimizer, k_per_layer, new_masks=None):
 
     The gradients must be dense: run the forward / backward inside ``ops.dense_weight_grad()``.  Per masked layer l,
     the k_per_layer[l] live weights of smallest |w| are dropped and as many pruned positions of largest |g| (the
-    just-dropped ones included) are grown; ties go to the lower flat index.  Grown weights and their momentum
-    (``optimizer.state[w]['momentum_buffer']`` when there is one) restart at 0; regrown dropped weights keep theirs.
+    just-dropped ones included) are grown; ties go to the lower flat index.  Grown weights and their optimizer state
+    (``momentum_buffer``, or AdamW's ``exp_avg`` and ``exp_avg_sq``, when there is one) restart at 0 in the same launch;
+    regrown dropped weights keep theirs.
     Masks, weights and momenta are updated in place (``mask_layers.mask_epoch()`` does not change).  Under
     torch.distributed every rank selects, rank 0's result is broadcast, every rank applies it.  ``new_masks``:
     scratch tensors of the masks' shapes to reuse.  Returns an int64 cuda tensor [layers, 2] of (dropped, grown)."""
@@ -246,9 +247,19 @@ def rigl_update(model: nn.Module, optimizer, k_per_layer, new_masks=None):
     counts = ops.rigl_select(ws, gs, ms, new_masks, k_per_layer)
     sync_masks_from_rank0_(new_masks)
     state = getattr(optimizer, "state", {}) if optimizer is not None else {}
-    bufs = [state[m.weight].get("momentum_buffer") if m.weight in state else None for m in layers]
-    ops.rigl_apply(ms, new_masks, ws, bufs)
+    per_layer = [state[m.weight] if m.weight in state else {} for m in layers]
+    # every per-element state the optimizer keeps (SGD: momentum_buffer; AdamW: exp_avg, exp_avg_sq; AdamW's
+    # per-parameter step is left alone); SGD, or no state at all, keeps the one-state apply
+    keys = [k for k in _RIGL_RESTART_KEYS if any(k in st for st in per_layer)] or ["momentum_buffer"]
+    states = [[st.get(k) for st in per_layer] for k in keys]
+    if len(keys) == 1:
+        ops.rigl_apply(ms, new_masks, ws, states[0])
+    else:
+        ops.rigl_apply_states(ms, new_masks, ws, states)
     return counts
+
+
+_RIGL_RESTART_KEYS = ("momentum_buffer", "exp_avg", "exp_avg_sq")
 
 
 def prune_the_model(cfg, harness, target_density: float) -> None:
