@@ -168,21 +168,32 @@ def test_mask_epoch_counts_new_mask_tensors():
     assert ml.mask_epoch() == e0 + 2 and "mask" in dict(m.named_buffers())
 
 
-def test_operand_planning_of_the_weight_shadow():
-    """Host-side layout decisions shared by the per-layer staging and the one-launch WeightStager."""
+def test_layer_plan_of_the_forward_and_the_weight_shadow():
+    """Host-side layout decisions shared by the masked layers' forward and the one-launch WeightStager:
+    ops.layer_plan gives (cin_p, cout_p, has_wd, wf_ld)."""
     from turboprune_b200 import ops
     assert ops.stem_geometry(3, 7, 7) == (3, 152)            # RGB 7x7 stem: 147 real columns, K padded to 8
     assert ops.stem_geometry(3, 3, 3) == (3, 32)             # CIFAR stem
     assert ops.stem_geometry(8, 3, 3) == (8, 72)
-    assert ops._operand_plan(64, 3, 7, 7) == (3, 64, False, 152)          # stem: no dgrad operand
-    assert ops._operand_plan(64, 64, 3, 3) == (64, 64, True, 576)
-    assert ops._operand_plan(96, 64, 3, 3) == (64, 128, True, 576)        # multi-tap backward walks Cout in 64-blocks
-    assert ops._operand_plan(1000, 2048, 1, 1) == (2048, 1000, True, 2048)
-    assert ops._operand_plan(10, 512, 1, 1) == (512, 16, True, 512)
-    assert ops._operand_plan(32, 12, 3, 3) == (64, 64, True, 576)         # 9..63 channels with k > 1: zero-padded to 64
-    assert ops._operand_plan(24, 16, 1, 1) == (16, 24, True, 16)
-    assert ops._operand_plan(10, 10, 1, 1) == (16, 16, True, 16)          # a 1x1 / linear needs 16-byte rows only
+    assert ops.layer_plan(64, 3, 7, 7) == (3, 64, False, 152)             # stem: no dgrad operand
+    assert ops.layer_plan(64, 64, 3, 3) == (64, 64, True, 576)
+    assert ops.layer_plan(96, 64, 3, 3) == (64, 128, True, 576)           # multi-tap backward walks Cout in 64-blocks
+    assert ops.layer_plan(1000, 2048, 1, 1) == (2048, 1000, True, 2048)
+    assert ops.layer_plan(10, 512, 1, 1) == (512, 16, True, 512)
+    assert ops.layer_plan(32, 12, 3, 3) == (64, 64, True, 576)            # 9..63 channels with k > 1: zero-padded to 64
+    assert ops.layer_plan(24, 16, 1, 1) == (16, 24, True, 16)
+    assert ops.layer_plan(10, 10, 1, 1) == (16, 16, True, 16)             # a 1x1 / linear needs 16-byte rows only
     assert ops.padded_cin(3, 1, 1) == 8 and ops.padded_cin(65, 3, 3) == 128 and ops.padded_cin(256, 3, 3) == 256
+    # the stem layout only serves a layer whose input needs no gradient; with one, the TMA layouts take its place
+    assert ops.layer_plan(64, 3, 7, 7).stem and not ops.layer_plan(64, 3, 7, 7, need_dx=True).stem
+    assert ops.layer_plan(64, 3, 7, 7, need_dx=True) == (64, 64, True, 3136)
+    assert ops.layer_plan(64, 8, 3, 3) == (8, 64, False, 72)
+    assert ops.layer_plan(64, 8, 3, 3, need_dx=True) == (64, 64, True, 576)
+    assert ops.layer_plan(10, 3, 1, 1) == (3, 10, False, 8)               # stem Cout is not padded
+    assert ops.layer_plan(10, 3, 1, 1, need_dx=True) == (8, 16, True, 8)
+    assert ops.layer_plan(64, 8, 1, 1) == ops.layer_plan(64, 8, 1, 1, need_dx=True) == (8, 64, True, 8)   # one row group
+    for shape in [(64, 64, 3, 3), (96, 64, 3, 3), (1000, 2048, 1, 1), (32, 12, 3, 3), (10, 10, 1, 1)]:
+        assert ops.layer_plan(*shape, need_dx=True) == ops.layer_plan(*shape)
 
 
 def test_device_resident_checkpoint_cache(tmp_path, monkeypatch):

@@ -364,11 +364,11 @@ HARNESS_CASES = [("resnet18", "cifar10", "ConvMask", 64), ("resnet50", "imagenet
                  ("vgg16", "cifar10", "ConvMask", 64), ("local_deit_small_patch16_224", "imagenet", "LinearMask", 16)]
 
 
-def _harness(case, tmp_path):
+def _harness(case, tmp_path, precision="float32"):
     from refshim import make_cfg, make_harness
     from turboprune_b200.utils import custom_models as cm, pruning_utils as pu
     model_name, data, mlt, batch = case
-    cfg = make_cfg(model_name, data, mask_layer_type=mlt, precision="float32")
+    cfg = make_cfg(model_name, data, mask_layer_type=mlt, precision=precision)
     cfg["optimizer_params"].update(lr=0.05, weight_decay=5e-4)
     torch.manual_seed(0)
     model = cm.CustomModel(cfg) if mlt == "LinearMask" else cm.TorchVisionModel(cfg)
@@ -415,6 +415,28 @@ def test_fp32_train_step_matches_oracle(dev, case, tmp_path, monkeypatch):
     assert not (set(rec.calls) & BF16_ENTRIES), sorted(set(rec.calls) & BF16_ENTRIES)
     assert "tp_conv_fprop_f32" in rec.calls and "tp_wgrad_split3" in rec.calls and "tp_conv_wgrad" in rec.calls
     assert dtypes <= {torch.float32, torch.int64}, dtypes
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("precision", ["bfloat16", "float32"])
+@pytest.mark.parametrize("case", HARNESS_CASES, ids=[c[0] for c in HARNESS_CASES])
+def test_train_step_consumes_the_weight_shadow(dev, case, precision, tmp_path, monkeypatch):
+    """In a train step every masked layer runs on the operands of the one-launch weight shadow: no layer stages its own
+    (tp_stage_weights / tp_stage_weights_f32), at either precision."""
+    from turboprune_b200 import _cabi
+    _, _, h = _harness(case, tmp_path, precision)
+    _, data, _, batch = case
+    size = 32 if data.startswith("cifar") else 224
+    g = torch.Generator().manual_seed(2)
+    x = torch.randn(batch, 3, size, size, generator=g)
+    t = torch.randint(0, 10, (batch,), generator=g)
+    rec = _Recorder(_cabi.load())
+    monkeypatch.setattr(_cabi, "_lib", rec)
+    h.train_step((x.cuda(), t.cuda()))
+    torch.cuda.synchronize()
+    batched = "tp_stage_weights_batched" if precision == "bfloat16" else "tp_stage_weights_batched_f32"
+    assert rec.calls.count(batched) == 1
+    assert not {"tp_stage_weights", "tp_stage_weights_f32"} & set(rec.calls), sorted(set(rec.calls))
 
 
 def _cpu_masked_forward(mod):

@@ -524,7 +524,7 @@ def test_cuda_graph_step_is_bit_identical_to_eager(dev, tmp_path):
         assert torch.equal(m1.weight, m2.weight) and bool((m2.weight.grad[m2.mask == 0] == 0).all())
 
 
-def test_batched_weight_staging_matches_per_layer(dev):
+def test_batched_weight_staging_matches_the_per_layer_plan(dev):
     """WeightStager: one launch writes the bf16(mask*w) fprop / dgrad operands of every layer (stem conv with 3
     channels, 3x3 and 1x1 convs, the fc) — bit-identical to the per-layer staging kernel; the pairs are consumed
     exactly once; a train step with the stager gives bit-identical weights to one without."""
@@ -547,7 +547,7 @@ def test_batched_weight_staging_matches_per_layer(dev):
         if w.dim() != 4:
             w = w.reshape(w.shape[0], w.shape[1], 1, 1); m = m.reshape(w.shape)
         cout, cin, r, s = w.shape
-        cin_p, cout_p, has_wd, wf_ld = ops._operand_plan(cout, cin, r, s)
+        cin_p, cout_p, has_wd, wf_ld = ops.layer_plan(cout, cin, r, s)
         wf, wd = ops.stage_weights(w.contiguous(), m.contiguous(), cin_p, has_wd, cout_p, wf_ld=wf_ld)
         got = ops.take_staged(l)
         assert got is not None and ops.take_staged(l) is None            # consumed exactly once

@@ -216,8 +216,7 @@ class BaseHarness:
         """A staged operand pair must never outlive its step (a layer skipped by this forward would otherwise feed the
         next eval / pruning forward bf16 weights from before optimizer.step())."""
         if self._stager is not None:
-            for l in self._stager.layers:
-                l.__dict__["_tp_staged"] = None
+            self._stager.drop()
 
     def test_step(self, batch):
         inputs, targets = batch

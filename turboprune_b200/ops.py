@@ -6,6 +6,7 @@ import ctypes
 import threading
 from contextlib import contextmanager
 from ctypes import c_void_p
+from typing import Callable, NamedTuple, Optional
 
 import torch
 
@@ -152,12 +153,12 @@ def grad_ready(*slots):
 # dW of a layer is needed by nobody before the gradient exchange / the optimizer, while dX is the critical path of the
 # backward pass.  With WGRAD_SIDE_STREAM the wgrad GEMM + finalize of every masked layer go to one side stream behind an
 # event of the compute stream; at small per-GPU batches (the 8-GPU operating point: 64 images) the kernels are one or two
-# waves each and the two chains fill each other's gaps.  The operands are kept alive until ``join_wgrad`` (the caching
+# waves each and the two chains fill each other's gaps.  The operands are marked as used by the side stream (the caching
 # allocator would otherwise hand their blocks to the next main-stream allocation while the side stream still reads them).
 # Off unless a caller that also joins turns it on (BaseHarness._step_body does, around its backward pass).
 WGRAD_SIDE_STREAM = False
 _wgrad_streams = {}
-_wgrad_keepalive = []
+_wgrad_pending = set()      # devices with weight gradients launched on the side stream since the last join
 
 
 def set_wgrad_side_stream(on: bool):
@@ -173,15 +174,12 @@ def _wgrad_stream(device):
 
 
 def join_wgrad(device=None):
-    """Make the current stream wait for every weight gradient launched on the side stream since the last join, and let go
-    of the operands kept alive for them.  Call after ``loss.backward()``, before anything consumes ``param.grad``."""
-    if not _wgrad_keepalive:
-        return
-    devs = {t[0].device for t in _wgrad_keepalive}
-    for d in devs:
+    """Make the current stream wait for every weight gradient launched on the side stream since the last join.  Call
+    after ``loss.backward()``, before anything consumes ``param.grad``."""
+    for d in _wgrad_pending:
         if device is None or d == device:
             torch.cuda.current_stream(d).wait_stream(_wgrad_stream(d))
-    _wgrad_keepalive.clear()
+    _wgrad_pending.clear()
 
 
 def _require_cuda(*tensors):
@@ -548,127 +546,119 @@ def padded_cin(cin, r, s):
     return _round_up(cin, 64 if r * s > 1 else 8)
 
 
-def _operand_plan(cout, cin, r, s):
-    """(cin_p, cout_p, has_wd, wf_ld) of the bf16 operand layouts a masked layer consumes in a train step (the
-    WeightStager's view): the stem layout for <= 8 input channels (explicit im2col, no input gradient), otherwise the
-    TMA layouts with the input channels padded to ``padded_cin``."""
-    if cin <= 8 and (cin % 8 != 0 or r * s > 1):
-        cg, kp = stem_geometry(cin, r, s)                    # stem: explicit im2col over padded channel groups, no dgrad
-        return cg, cout, False, kp
+class LayerPlan(NamedTuple):
+    """Operand layout of a masked layer (see ``layer_plan``)."""
+    cin_p: int          # input channels as laid out: padded to ``padded_cin``; for the stem, cg = cin channels per tap
+    cout_p: int         # output channels the backward GEMMs walk (cout for the stem)
+    has_wd: bool        # a dgrad operand exists: False exactly for the stem
+    wf_ld: int          # row length of the fprop operand: taps * cin_p; for the stem, its K padded to 8 (kp)
+
+    @property
+    def stem(self):
+        return not self.has_wd
+
+
+def layer_plan(cout, cin, r, s, need_dx=False):
+    """The operand layout of a masked layer with weight [cout, cin, r, s].  <= 8 input channels that do not fill one
+    16-byte row (or sit under a multi-tap filter) and no input gradient wanted (the RGB stem): explicit im2col over
+    ``stem_geometry`` columns and a plain GEMM, with no dgrad operand.  Everything else: the TMA layouts, the input
+    channels zero-padded to ``padded_cin`` and Cout padded for the backward GEMMs, which walk it in 64-channel blocks
+    per tap when the filter has more than one tap.  The WeightStager plans with ``need_dx=False``."""
+    if cin <= 8 and (cin % 8 != 0 or r * s > 1) and not need_dx:
+        cg, kp = stem_geometry(cin, r, s)
+        return LayerPlan(cg, cout, False, kp)
     cin_p = padded_cin(cin, r, s)
-    return cin_p, _round_up(cout, 64 if r * s > 1 else 8), True, r * s * cin_p
+    return LayerPlan(cin_p, _round_up(cout, 64 if r * s > 1 else 8), True, r * s * cin_p)
+
+
+def _layer_descs(plan, weight_shape, x_shape, stride, padding):
+    """(conv, fprop, wgrad, dgrad) descriptors of a masked layer run with ``plan``.  conv: the convolution over the input
+    as laid out.  The stem runs fprop and wgrad as one GEMM over the im2col rows and has no dgrad; the TMA wgrad walks
+    Cout padded to cout_p, and the dgrad also writes only the real input channels."""
+    cout, cin, r, s = weight_shape
+    n, _, h, w = x_shape
+    desc = make_desc(n, h, w, plan.cin_p, cout, r, s, stride, padding)
+    if plan.stem:
+        gdesc = _cabi.ConvDesc(n * desc.p * desc.q, 1, 1, plan.wf_ld, cout, 1, 1, 1, 1, 0, 0, 1, 1)
+        return desc, gdesc, gdesc, None
+    padded = lambda c: _cabi.ConvDesc(n, h, w, c, plan.cout_p, r, s, desc.stride_h, desc.stride_w, desc.pad_h,
+                                      desc.pad_w, desc.p, desc.q)
+    wdesc = desc if plan.cout_p == cout else padded(plan.cin_p)
+    return desc, desc, wdesc, wdesc if cin == plan.cin_p else padded(cin)
+
+
+def _shape4(w):
+    return tuple(w.shape) if w.dim() == 4 else (w.shape[0], w.shape[1], 1, 1)   # Linear [out, in] / Conv1d(k=1) [out, in, 1]
+
+
+class Staged(NamedTuple):
+    """The operands a ``WeightStager`` left for one layer's next forward, and the plan they are laid out for."""
+    wf: torch.Tensor
+    wd: Optional[torch.Tensor]
+    plan: LayerPlan
+
+
+class _Shadow:
+    """The weight shadow at one precision: persistent operand buffers of every layer the batched kernel stages (bf16
+    also: the K-block occupancy masks of all layers in ONE buffer, zeroed by a single memset node per step), the
+    StageItem table over them and the kernel's workspace, which caches the table on the device."""
+
+    def __init__(self, layers, dtype):
+        dev = layers[0].weight.device
+        self.staged = []                   # (layer, Staged); a layer left out stages its own operands in its forward
+        for l in layers:
+            w = l.weight
+            if not w.is_cuda or w.dtype != torch.float32 or not w.is_contiguous():
+                continue
+            cout, cin, r, s = _shape4(w)
+            plan = layer_plan(cout, cin, r, s)
+            wf = torch.zeros(cout, plan.wf_ld, dtype=dtype, device=dev)
+            wd = torch.zeros(cin, r * s * plan.cout_p, dtype=dtype, device=dev) if plan.has_wd else None
+            self.staged.append((l, Staged(wf, wd, plan)))
+        self.kmask_all = None
+        if dtype == torch.bfloat16:
+            sizes = []
+            for l, st in self.staged:
+                sf, sd = kmask_shapes(*_shape4(l.weight), st.plan.wf_ld, st.plan.cout_p)
+                sizes.append((sf[0] * sf[1] + 1, sd[0] * sd[1] + 1 if st.wd is not None else 0))
+            self.kmask_all = torch.zeros(max(sum(f + d for f, d in sizes), 1), dtype=torch.int32, device=dev)
+            off = 0
+            for (_, st), (f, d) in zip(self.staged, sizes):
+                st.wf.kmask = self.kmask_all[off:off + f]
+                if st.wd is not None:
+                    st.wd.kmask = self.kmask_all[off + f:off + f + d]
+                off += f + d
+        lib = _cabi.load()
+        self.ws = torch.empty(max(int(lib.tp_stage_batched_workspace_bytes(len(layers))), 256), dtype=torch.uint8, device=dev)
+        self.key = self.items = None
+
+    def set_table(self, key):
+        items = (_cabi.StageItem * len(self.staged))()
+        for it, (l, st) in zip(items, self.staged):
+            it.w = l.weight.data_ptr(); it.mask = l.mask.data_ptr()
+            it.wf = st.wf.data_ptr(); it.wd = st.wd.data_ptr() if st.wd is not None else None
+            it.cout, it.cin, it.r, it.s = _shape4(l.weight)
+            it.cin_p, it.cout_p, it.wf_ld = st.plan.cin_p, st.plan.cout_p, st.plan.wf_ld
+            kf, kd = getattr(st.wf, "kmask", None), getattr(st.wd, "kmask", None)
+            it.kmask_f = kf.data_ptr() if kf is not None else None
+            it.kmask_d = kd.data_ptr() if kd is not None else None
+        self.items, self.key = items, key
 
 
 class WeightStager:
-    """bf16 "weight shadow" of a whole model, refreshed by ONE launch per optimizer step (SURVEY.md §8(f) row 2).
+    """"Weight shadow" of a whole model, refreshed by ONE launch per optimizer step (SURVEY.md §8(f) row 2).
 
-    ``stage()`` writes bf16(mask * w) of every masked layer into persistent fprop / dgrad operand buffers and hands
-    them to the layers; each layer consumes its pair in its next forward (exactly once) instead of launching its own
-    staging kernel — the reference's per-layer ``mask * weight`` + autocast cast (mask_layers.py:25-34) become one
-    kernel per step.  Call it right before the training forward; a forward without a preceding ``stage()`` (eval,
-    pruning scores) stages per layer as before.  Pointers are re-checked every call (pruning replaces mask tensors),
-    the device table is only re-uploaded when they changed, so the call is CUDA-graph capturable after a warm-up step."""
+    ``stage()`` writes mask * w of every masked layer, at the current precision (bf16, or float32 inside
+    ``compute_precision(torch.float32)``), into persistent fprop / dgrad operand buffers and hands them to the layers;
+    each layer consumes its ``Staged`` pair in its next forward (exactly once) instead of launching its own staging
+    kernel — the reference's per-layer ``mask * weight`` + autocast cast (mask_layers.py:25-34) become one kernel per
+    step.  Call it right before the training forward; a forward without a preceding ``stage()`` (eval, pruning scores)
+    stages per layer.  Pointers are re-checked every call (pruning replaces mask tensors), the device table is only
+    re-uploaded when they changed, so the call is CUDA-graph capturable after a warm-up step."""
 
     def __init__(self, layers):
-        self.layers = [l for l in layers]
-        self._key = None
-        self._bufs = None
-        self._items = None
-        self._ws = None
-
-    @staticmethod
-    def _shape4(layer):
-        w = layer.weight
-        if w.dim() == 4:
-            return tuple(w.shape)
-        return (w.shape[0], w.shape[1], 1, 1)                 # Linear [out, in] / Conv1d(k=1) [out, in, 1]
-
-    def _rebuild(self, key):
-        dev = self.layers[0].weight.device
-        if self._bufs is None:
-            self._bufs = []
-            for l in self.layers:
-                cout, cin, r, s = self._shape4(l)
-                plan = _operand_plan(cout, cin, r, s)
-                if plan is None or not l.weight.is_cuda or l.weight.dtype != torch.float32 or not l.weight.is_contiguous():
-                    self._bufs.append(None)
-                    continue
-                cin_p, cout_p, has_wd, wf_ld = plan
-                wf = torch.zeros(cout, wf_ld, dtype=torch.bfloat16, device=dev)
-                wd = torch.zeros(cin, r * s * cout_p, dtype=torch.bfloat16, device=dev) if has_wd else None
-                self._bufs.append((wf, wd, cin_p, cout_p))
-            # K-block occupancy masks of all layers in ONE buffer (zeroed by a single memset node per step)
-            shapes = []
-            for l, b in zip(self.layers, self._bufs):
-                if b is None:
-                    shapes.append(None); continue
-                cout, cin, r, s = self._shape4(l)
-                shapes.append(kmask_shapes(cout, cin, r, s, b[0].shape[1], b[3]))
-            total = sum(sf[0] * sf[1] + 1 + ((sd[0] * sd[1] + 1) if b[1] is not None else 0)
-                        for (sh, b) in zip(shapes, self._bufs) if sh is not None for sf, sd in [sh])
-            self._kmask_all = torch.zeros(max(total, 1), dtype=torch.int32, device=dev)
-            off = 0
-            for sh, b in zip(shapes, self._bufs):
-                if sh is None:
-                    continue
-                sf, sd = sh
-                b[0].kmask = self._kmask_all[off:off + sf[0] * sf[1] + 1]; off += sf[0] * sf[1] + 1
-                if b[1] is not None:
-                    b[1].kmask = self._kmask_all[off:off + sd[0] * sd[1] + 1]; off += sd[0] * sd[1] + 1
-        live = [(l, b) for l, b in zip(self.layers, self._bufs) if b is not None]
-        items = (_cabi.StageItem * len(live))()
-        for it, (l, (wf, wd, cin_p, cout_p)) in zip(items, live):
-            cout, cin, r, s = self._shape4(l)
-            it.w = l.weight.data_ptr(); it.mask = l.mask.data_ptr()
-            it.wf = wf.data_ptr(); it.wd = wd.data_ptr() if wd is not None else None
-            it.cout, it.cin, it.r, it.s, it.cin_p, it.cout_p, it.wf_ld = cout, cin, r, s, cin_p, cout_p, wf.shape[1]
-            it.kmask_f = wf.kmask.data_ptr()
-            it.kmask_d = wd.kmask.data_ptr() if wd is not None else None
-        self._items, self._live, self._key = items, live, key
-        if self._ws is None:
-            lib = _cabi.load()
-            self._ws = torch.empty(max(int(lib.tp_stage_batched_workspace_bytes(len(self.layers))), 256), dtype=torch.uint8, device=dev)
-
-    def _stage_f32(self, key):
-        """fp32 operands (inside ``compute_precision(torch.float32)``): the same layouts as fp32, their own persistent
-        buffers and pointer table, no occupancy masks."""
-        lib = _cabi.load()
-        st = self.__dict__.setdefault("_f32", {})
-        if st.get("key") != key:
-            dev = self.layers[0].weight.device
-            if "bufs" not in st:
-                bufs = []
-                for l in self.layers:
-                    cout, cin, r, s = self._shape4(l)
-                    if not l.weight.is_cuda or l.weight.dtype != torch.float32 or not l.weight.is_contiguous():
-                        bufs.append(None); continue
-                    cin_p, cout_p, has_wd, wf_ld = _operand_plan(cout, cin, r, s)
-                    wf = torch.zeros(cout, wf_ld, dtype=torch.float32, device=dev)
-                    wd = torch.zeros(cin, r * s * cout_p, dtype=torch.float32, device=dev) if has_wd else None
-                    bufs.append((wf, wd, cin_p, cout_p))
-                st["bufs"] = bufs
-                st["ws"] = torch.empty(max(int(lib.tp_stage_batched_workspace_bytes(len(self.layers))), 256), dtype=torch.uint8,
-                                       device=dev)
-            live = [(l, b) for l, b in zip(self.layers, st["bufs"]) if b is not None]
-            items = (_cabi.StageItem * len(live))()
-            for it, (l, (wf, wd, cin_p, cout_p)) in zip(items, live):
-                cout, cin, r, s = self._shape4(l)
-                it.w = l.weight.data_ptr(); it.mask = l.mask.data_ptr()
-                it.wf = wf.data_ptr(); it.wd = wd.data_ptr() if wd is not None else None
-                it.cout, it.cin, it.r, it.s, it.cin_p, it.cout_p, it.wf_ld = cout, cin, r, s, cin_p, cout_p, wf.shape[1]
-                it.kmask_f = it.kmask_d = None
-            st.update(key=key, items=items, live=live, cached=False)
-        if not st["live"]:
-            return
-        dev = self.layers[0].weight.device
-        with torch.cuda.device(dev):
-            rc = lib.tp_stage_weights_batched_f32(st["items"], len(st["live"]), int(st["cached"]), c_void_p(st["ws"].data_ptr()),
-                                                  st["ws"].numel(), _cabi.stream_ptr(dev))
-        _cabi.check(rc, "tp_stage_weights_batched_f32")
-        st["cached"] = True
-        _count()
-        for l, (wf, wd, _, _) in st["live"]:
-            l.__dict__["_tp_staged"] = (wf, wd)
+        self.layers = list(layers)
+        self._shadows = {}                 # precision -> _Shadow
 
     def stage(self):
         lib = _cabi.load()
@@ -676,22 +666,39 @@ class WeightStager:
             if l.mask.device != l.weight.device or l.mask.dtype != torch.float32 or not l.mask.is_contiguous():
                 l.mask = l.mask.to(device=l.weight.device, dtype=torch.float32).contiguous()
         key = tuple((l.weight.data_ptr(), l.mask.data_ptr()) for l in self.layers)
-        if current_precision() == torch.float32:
-            return self._stage_f32(key)
-        cached = key == self._key
+        dtype = current_precision()
+        sh = self._shadows.get(dtype)
+        if sh is None:
+            sh = self._shadows[dtype] = _Shadow(self.layers, dtype)
+        cached = key == sh.key
         if not cached:
-            self._rebuild(key)
-        if not len(self._live):
+            sh.set_table(key)
+        if not sh.staged:
             return
         dev = self.layers[0].weight.device
         with torch.cuda.device(dev):
-            rc = lib.tp_stage_weights_batched(self._items, len(self._live), int(cached), c_void_p(self._kmask_all.data_ptr()),
-                                              self._kmask_all.numel() * 4, c_void_p(self._ws.data_ptr()),
-                                              self._ws.numel(), _cabi.stream_ptr(dev))
-        _cabi.check(rc, "tp_stage_weights_batched")
+            if dtype == torch.bfloat16:
+                rc = lib.tp_stage_weights_batched(sh.items, len(sh.staged), int(cached), c_void_p(sh.kmask_all.data_ptr()),
+                                                  sh.kmask_all.numel() * 4, c_void_p(sh.ws.data_ptr()), sh.ws.numel(),
+                                                  _cabi.stream_ptr(dev))
+                _cabi.check(rc, "tp_stage_weights_batched")
+            else:
+                rc = lib.tp_stage_weights_batched_f32(sh.items, len(sh.staged), int(cached), c_void_p(sh.ws.data_ptr()),
+                                                      sh.ws.numel(), _cabi.stream_ptr(dev))
+                _cabi.check(rc, "tp_stage_weights_batched_f32")
         _count()
-        for l, (wf, wd, _, _) in self._live:
-            l.__dict__["_tp_staged"] = (wf, wd)
+        for l, st in sh.staged:
+            l.__dict__["_tp_staged"] = st
+
+    def shadow(self, dtype=torch.bfloat16):
+        """(layer, Staged) of every layer ``stage()`` covers at ``dtype``; empty before the first ``stage()`` there."""
+        sh = self._shadows.get(dtype)
+        return list(sh.staged) if sh is not None else []
+
+    def drop(self):
+        """Take back what the last ``stage()`` handed out and no forward consumed."""
+        for l in self.layers:
+            l.__dict__.pop("_tp_staged", None)
 
 
 def skipped_block_report(stager):
@@ -699,24 +706,18 @@ def skipped_block_report(stager):
     (never loaded / multiplied).  For iid unstructured masks this is ~0 at any density a 64x64 block survives
     (SURVEY.md Appendix B); dead filters / dead input channels are what produces skippable blocks."""
     rows, empty, total = [], 0, 0
-    for l, b in zip(stager.layers, stager._bufs):
-        if b is None or getattr(b[0], "kmask", None) is None:
-            continue
-        e, t = kblock_occupancy(b[0].kmask, b[0].shape[1])
+    for l, st in stager.shadow(torch.bfloat16):
+        e, t = kblock_occupancy(st.wf.kmask, st.wf.shape[1])
         rows.append((type(l).__name__, tuple(l.weight.shape), e, t))
         empty += e; total += t
     return {"empty_blocks": empty, "total_blocks": total, "fraction": empty / max(total, 1), "layers": rows}
 
 
 def take_staged(layer):
-    """The (wf, wd) pair a ``WeightStager`` left for this layer's next forward, or None; consumed exactly once.  A pair
-    staged at the other precision than the current one is dropped."""
-    st = layer.__dict__.get("_tp_staged")
-    if st is not None:
-        layer.__dict__["_tp_staged"] = None
-        if st[0].dtype != (torch.float32 if current_precision() == torch.float32 else torch.bfloat16):
-            return None
-    return st
+    """The ``Staged`` operands a ``WeightStager`` left for this layer's next forward, or None; consumed exactly once.
+    Operands staged at another precision than the current one are dropped."""
+    st = layer.__dict__.pop("_tp_staged", None)
+    return st if st is not None and st.wf.dtype == current_precision() else None
 
 
 def to_nhwc_bf16(x, c_pad):
@@ -733,19 +734,6 @@ def to_nhwc_bf16(x, c_pad):
         rc = lib.tp_to_nhwc_bf16(c_void_p(x.data_ptr()), 0 if x.dtype == torch.float32 else 1, sn, sc, sh, sw,
                                  n, c, h, w, c_void_p(out.data_ptr()), c_pad, _cabi.stream_ptr(x.device))
     _cabi.check(rc, "tp_to_nhwc_bf16")
-    _count()
-    return out
-
-
-def im2col_c8(x_nhwc8, desc, kp):
-    lib = _cabi.load()
-    n, h, w, _ = x_nhwc8.shape
-    out = torch.empty(n * desc.p * desc.q, kp, dtype=torch.bfloat16, device=x_nhwc8.device)
-    with torch.cuda.device(x_nhwc8.device):
-        rc = lib.tp_im2col_c8(c_void_p(x_nhwc8.data_ptr()), n, h, w, desc.r, desc.s, desc.stride_h, desc.stride_w,
-                              desc.pad_h, desc.pad_w, desc.p, desc.q, c_void_p(out.data_ptr()), kp,
-                              _cabi.stream_ptr(x_nhwc8.device))
-    _cabi.check(rc, "tp_im2col_c8")
     _count()
     return out
 
@@ -971,201 +959,120 @@ def conv_wgrad_f32(desc, xs, dys, mask4d, cin_real, dw_out=None):
     return dw
 
 
-def _fp32_forward(ctx, x, weight, mask, bias, stride, padding, want_skip, grad_slots, staged, want_stats):
+def _check_f32(x, want_skip, want_stats):
     if want_skip or want_stats:
         raise RuntimeError("masked_conv2d at float32: the skip-gradient and BatchNorm-statistics epilogues exist in bf16 "
                            "only (a float32 model runs unfused)")
     if x.dtype != torch.float32:
         raise TypeError(f"masked layers at float32 need fp32 activations, got {x.dtype}")
-    ctx.set_materialize_grads(False)
-    ctx.f32 = True
-    ctx.grad_slots = grad_slots
-    cout, cin, r, s = weight.shape
-    n, _, h, w = x.shape
-    need_dx = ctx.needs_input_grad[0]
-    w32 = weight.detach().contiguous()
-    m32 = mask.detach().contiguous()
-    cin_p = padded_cin(cin, r, s)
-    small_c = cin <= 8 and cin_p != cin and not need_dx
-    desc = make_desc(n, h, w, cin_p if not small_c else cin, cout, r, s, stride, padding)
-    cout_p = _round_up(cout, 64 if (r * s > 1 and not small_c) else 8)
-    y = empty_cl(n, cout, desc.p, desc.q, x.device, torch.float32)
-    if small_c:
-        cg, kp = stem_geometry(cin, r, s)
-        xg = im2col_stem_f32(x, desc, kp, cg)
-        gdesc = _cabi.ConvDesc(n * desc.p * desc.q, 1, 1, kp, cout, 1, 1, 1, 1, 0, 0, 1, 1)
-        wf = staged[0] if staged is not None and staged[0].shape == (cout, kp) else stage_weights_f32(w32, m32, cg, False, wf_ld=kp)[0]
-        conv_fprop_f32(gdesc, xg, wf, bias, out=y)
-        ctx.mode = "stem"
-        ctx.gdesc = gdesc
-        ctx.save_for_backward(xg, m32)
-    else:
-        xn = to_nhwc_f32(x, cin_p)
-        if (staged is not None and staged[0].shape == (cout, r * s * cin_p)
-                and (not need_dx or (staged[1] is not None and staged[1].shape == (cin, r * s * cout_p)))):
-            wf, wd = staged
-        else:
-            wf, wd = stage_weights_f32(w32, m32, cin_p, need_dx, cout_p)
-        conv_fprop_f32(desc, xn, wf, bias, out=y)
-        ctx.mode = "conv"
-        ctx.save_for_backward(xn, m32, wd)
-    ctx.desc = desc
-    ctx.cin = cin
-    ctx.has_bias = bias is not None
-    ctx.cout_p = cout_p
-    return y
 
 
-def _fp32_backward(ctx, dy):
-    desc = ctx.desc
-    rest = (None,) * 7                      # stride, padding, want_skip, grad_slots, staged, want_stats, bn_src
-    if dy is None:
-        return (None, None, None, None) + rest
-    cout = desc.cout
-    need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
-    need_db = ctx.has_bias and ctx.needs_input_grad[3]
-    if dy.dtype != torch.float32:
-        dy = dy.float()
-    dx = dw = db = None
-    if ctx.mode == "stem":
-        xg, m32 = ctx.saved_tensors
-        if need_dw:
-            r, s = desc.r, desc.s
-            cin = m32.shape[1]
-            rows, kp = xg.shape
-            gd = ctx.gdesc
-            # dy [N, cout, P, Q] splits to NHWC [3N, P, Q, cout]: the rows of the im2col matrix, three times over
-            xs, dys = split_stacks(gd, xg.view(rows, kp, 1, 1), dy, cout)
-            ones = torch.ones(cout, kp, dtype=torch.float32, device=xg.device)
-            dwm = conv_wgrad_f32(gd, xs, dys, ones.view(cout, kp, 1, 1), kp)
-            cg = stem_geometry(cin, r, s)[0]
-            dw = dwm[:, :r * s * cg].reshape(cout, r * s, cg)[:, :, :cin].permute(0, 2, 1).reshape(cout, cin, r, s)
-            if not ctx.dense:
-                dw = dw * m32
-    else:
-        xn, m32, wd = ctx.saved_tensors
-        if ctx.dense:
-            m32 = _ones_like_mask(m32)
-        cin = ctx.cin
-        ddesc = desc
-        if ctx.cout_p != cout:
-            ddesc = _cabi.ConvDesc(desc.n, desc.h, desc.w, desc.cin, ctx.cout_p, desc.r, desc.s, desc.stride_h,
-                                   desc.stride_w, desc.pad_h, desc.pad_w, desc.p, desc.q)
-        if need_dx:
-            dyn = to_nhwc_f32(dy, ctx.cout_p)
-            xdesc = ddesc if cin == desc.cin else _cabi.ConvDesc(desc.n, desc.h, desc.w, cin, ctx.cout_p, desc.r, desc.s,
-                                                                  desc.stride_h, desc.stride_w, desc.pad_h, desc.pad_w,
-                                                                  desc.p, desc.q)
-            dx = conv_dgrad_f32(xdesc, dyn, wd).permute(0, 3, 1, 2)
-        if need_dw:
-            # the stacks are written on the current stream; the GEMM may run on the side stream, which then owns them
-            xs, dys = split_stacks(ddesc, xn.permute(0, 3, 1, 2), dy, ctx.cout_p)
-            if ctx.cout_p != cout:
-                m_p = torch.zeros(ctx.cout_p, *m32.shape[1:], dtype=torch.float32, device=m32.device)
-                m_p[:cout] = m32
-                dw = conv_wgrad_f32(ddesc, xs, dys, m_p, cin)[:cout].contiguous()
-            else:
-                ws_ = ctx.grad_slots[0] if ctx.grad_slots is not None else None
-                direct_w = ws_ is not None and ws_.is_contiguous() and ws_.numel() == m32.numel()
-                if WGRAD_SIDE_STREAM and direct_w:
-                    dev = xn.device
-                    cur, side = torch.cuda.current_stream(dev), _wgrad_stream(dev)
-                    ev = torch.cuda.Event(); ev.record(cur)
-                    side.wait_event(ev)
-                    with torch.cuda.stream(side):
-                        conv_wgrad_f32(desc, xs, dys, m32, cin, dw_out=ws_)
-                        grad_ready(ws_)
-                    # freed as soon as this layer's GEMM is done, not at the join: 6 B per element of x and dy
-                    xs.record_stream(side); dys.record_stream(side); m32.record_stream(side)
-                    _wgrad_keepalive.append((ws_,))        # join_wgrad() waits for the side stream while anything is pending
-                else:
-                    dw = conv_wgrad_f32(desc, xs, dys, m32, cin, dw_out=ws_ if direct_w else None)
-                    if direct_w:
-                        dw = None
-                        grad_ready(ws_)
-    if need_db:
-        db = dy.sum(dim=(0, 2, 3))
-    return (dx, dw, None, db) + rest
+class _Precision(NamedTuple):
+    """What a masked layer does differently at each compute precision; ``MaskedConv2dFn`` is written once against it."""
+    act: torch.dtype                # activations, operands and input gradients
+    check: Callable                 # (x, want_skip, want_stats): raises for what this precision cannot run
+    stage: Callable                 # per-layer staging, as ``stage_weights``
+    nhwc: Callable                  # (x [N, C, H, W], c_pad) -> NHWC
+    im2col: Callable                # the stem's im2col, as ``im2col_stem``
+    fprop: Callable                 # (desc, x, wf, bias, out=y)
+    dy: Callable                    # (dy, cout_p): the form of dy the backward works from
+    dgrad: Callable                 # (desc, dy in that form, wd, addend, kmask) -> NHWC dx
+    wgrad_operands: Callable        # (desc, x as logical NCHW, dy in that form) -> the GEMM operands, made on the current stream
+    wgrad: Callable                 # (desc, x, dy, mask, cin_real, want_db, dw_out, db_out, kmask) -> (dw, db)
+    colsum_db: bool                 # wgrad also forms the bias gradient, as the column sums of dy
+
+
+_PRECISIONS = {
+    # dy laid out once as NHWC bf16; one conv_wgrad, the bias gradient from its column sums
+    torch.bfloat16: _Precision(
+        act=torch.bfloat16, check=lambda x, want_skip, want_stats: None, stage=stage_weights, nhwc=to_nhwc_bf16,
+        im2col=im2col_stem, fprop=conv_fprop, dy=to_nhwc_bf16, dgrad=conv_dgrad,
+        wgrad_operands=lambda desc, x, dy: (x, dy), wgrad=conv_wgrad, colsum_db=True),
+    # dy stays fp32 NCHW: dgrad lays it out, the weight gradient is one conv_wgrad over the split stacks of 3N images,
+    # and the bias gradient is dy.sum in fp32
+    torch.float32: _Precision(
+        act=torch.float32, check=_check_f32, stage=stage_weights_f32, nhwc=to_nhwc_f32, im2col=im2col_stem_f32,
+        fprop=conv_fprop_f32, dy=lambda dy, c_pad: dy.float(),
+        dgrad=lambda desc, dy, wd, addend, kmask: conv_dgrad_f32(desc, to_nhwc_f32(dy, desc.cout), wd),
+        wgrad_operands=lambda desc, x, dy: split_stacks(desc, x, dy, desc.cout),
+        wgrad=lambda desc, xs, dys, mask, cin, want_db, dw_out=None, db_out=None, kmask=None:
+            (conv_wgrad_f32(desc, xs, dys, mask, cin, dw_out=dw_out), None),
+        colsum_db=False),
+}
+
+
+def _on_wgrad_stream(fn, *operands):
+    """``fn()`` on the side stream, behind an event of the current stream.  Every operand is marked as in use by the side
+    stream, so the caching allocator hands its block to no other allocation before the side stream is done with it: the
+    operands are freed as soon as this GEMM is done, not at ``join_wgrad``."""
+    dev = operands[0].device
+    side = _wgrad_stream(dev)
+    ev = torch.cuda.Event(); ev.record(torch.cuda.current_stream(dev))
+    side.wait_event(ev)
+    with torch.cuda.stream(side):
+        out = fn()
+    for t in operands:
+        t.record_stream(side)
+    _wgrad_pending.add(dev)
+    return out
 
 
 class MaskedConv2dFn(torch.autograd.Function):
-    """y = conv2d(x, mask*w, b) with bf16 tensor-core operands and fp32 accumulation.
+    """y = conv2d(x, mask*w, b) with tensor-core operands and fp32 accumulation, at the current compute precision.
 
     Replaces ``F.conv2d(x, mask * weight, ...)`` under bf16 autocast (reference
     utils/mask_layers.py:23-34 executed inside base_harness.py:121-125) and its autograd
     backward: dX = dgrad(dY, mask*w), dW = mask * wgrad(x, dY) in fp32, db = sum dY.
-    Activations stay NHWC bf16 (logical NCHW tensors with channels_last strides).
+    Activations stay NHWC (logical NCHW tensors with channels_last strides), bf16 or fp32.
     """
 
     @staticmethod
     def forward(ctx, x, weight, mask, bias, stride, padding, want_skip=False, grad_slots=None, staged=None, want_stats=False,
                 bn_src=None):
         _require_cuda(x, weight, mask)
-        ctx.dense = dense_grad_enabled()                  # read once, like the precision: dW = wgrad(x, dy), unmasked
-        if current_precision() == torch.float32:        # read once; backward follows ctx.f32
-            return _fp32_forward(ctx, x, weight, mask, bias, stride, padding, want_skip, grad_slots, staged, want_stats)
+        P = ctx.prec = _PRECISIONS[current_precision()]    # read once, like dense: backward runs on autograd's thread
+        P.check(x, want_skip, want_stats)
+        ctx.dense = dense_grad_enabled()                  # dW = wgrad(x, dy), unmasked
         ctx.set_materialize_grads(False)
-        ctx.bn_src = None
         ctx.want_skip = want_skip
-        ctx.want_stats = want_stats
-        stats = None
         # (w_slot, b_slot): persistent arena slots; when given, backward writes dW / db there and returns None for
         # them (no AccumulateGrad add kernel; the slot IS param.grad)
         ctx.grad_slots = grad_slots
         cout, cin, r, s = weight.shape
-        n, _, h, w = x.shape
+        n = x.shape[0]
         need_dx = ctx.needs_input_grad[0]
-        w32 = weight.detach().contiguous()
         m32 = mask.detach().contiguous()
-        cin_p = padded_cin(cin, r, s)
-        # <= 8 input channels and no input gradient wanted (the RGB stem): explicit im2col + plain GEMM, K = taps * cin.
-        # Everything else goes through the TMA layouts with the channels zero-padded to cin_p.
-        small_c = cin <= 8 and cin_p != cin and not need_dx
-        desc = make_desc(n, h, w, cin_p if not small_c else cin, cout, r, s, stride, padding)
-        # the backward GEMMs contract over Cout: filters larger than 1x1 walk it in 64-channel blocks per tap
-        cout_p = _round_up(cout, 64 if (r * s > 1 and not small_c) else 8)    # (the stem path is a plain GEMM over im2col)
-        if small_c:
-            # stem conv: cg = cin channels per tap, explicit im2col, then a plain GEMM
-            cg, kp = stem_geometry(cin, r, s)
-            xg = im2col_stem(x, desc, kp, cg)
-            gdesc = _cabi.ConvDesc(n * desc.p * desc.q, 1, 1, kp, cout, 1, 1, 1, 1, 0, 0, 1, 1)
-            if staged is not None and staged[0].shape == (cout, kp):
-                wf, wd = staged
-            else:
-                wf, wd = stage_weights(w32, m32, cg, False, wf_ld=kp)
-            y = empty_cl(n, cout, desc.p, desc.q, x.device)
-            if want_stats:
-                _, stats = conv_fprop(gdesc, xg, wf, bias, out=y, want_stats=True)
-            else:
-                conv_fprop(gdesc, xg, wf, bias, out=y)
-            ctx.mode = "stem"
-            ctx.gdesc = gdesc
-            ctx.save_for_backward(xg, m32)
+        plan = ctx.plan = layer_plan(cout, cin, r, s, need_dx)
+        desc, fdesc, ctx.wdesc, ctx.xdesc = _layer_descs(plan, weight.shape, x.shape, stride, padding)
+        if plan.stem:
+            xin = P.im2col(x, desc, plan.wf_ld, plan.cin_p)
         else:
-            xn = to_nhwc_bf16(x, cin_p)      # channels cin..cin_p are zero (and so are the staged weights there)
-            if (staged is not None and staged[0].shape == (cout, r * s * cin_p)
-                    and (not need_dx or (staged[1] is not None and staged[1].shape == (cin, r * s * cout_p)))):
-                wf, wd = staged              # refreshed by WeightStager.stage() for this step (one launch for all layers)
-            else:
-                wf, wd = stage_weights(w32, m32, cin_p, need_dx, cout_p)
-            y = empty_cl(n, cout, desc.p, desc.q, x.device)
-            if want_stats:
-                _, stats = conv_fprop(desc, xn, wf, bias, out=y, want_stats=True)
-            else:
-                conv_fprop(desc, xn, wf, bias, out=y)
-            ctx.mode = "conv"
-            ctx.save_for_backward(xn, m32, wd)
-            # x is the output of a fused BatchNorm+ReLU (no residual): this layer's dgrad can do that BatchNorm's backward
-            # reduction in its epilogue (stride 1, no channel padding, the NHWC buffers line up)
-            if (bn_src is not None and BN_BWD_FUSION and need_dx and not want_skip and stride == (1, 1) and cin_p == cin
-                    and bn_src[0].shape == xn.shape):
-                ctx.bn_src = bn_src
-            ctx.wd_kmask = getattr(wd, "kmask", None) if wd is not None else None     # attributes do not survive save_for_backward
-            ctx.wf_kmask = getattr(wf, "kmask", None)                                  # wgrad skips tiles under all-zero mask blocks
+            xin = P.nhwc(x, plan.cin_p)      # channels cin..cin_p are zero (and so are the staged weights there)
+        if staged is not None and staged.plan == plan:
+            wf, wd = staged.wf, staged.wd    # refreshed by WeightStager.stage() for this step (one launch for all layers)
+        else:
+            # nothing staged (eval, pruning scores), or a stem layout for a layer whose input needs a gradient here
+            wf, wd = P.stage(weight.detach().contiguous(), m32, plan.cin_p, need_dx, plan.cout_p,
+                             wf_ld=plan.wf_ld if plan.stem else 0)
+        y = empty_cl(n, cout, desc.p, desc.q, x.device, P.act)
+        stats = None
+        if want_stats:
+            _, stats = conv_fprop(fdesc, xin, wf, bias, out=y, want_stats=True)
+        else:
+            P.fprop(fdesc, xin, wf, bias, out=y)
+        # x is the output of a fused BatchNorm+ReLU (no residual): this layer's dgrad can do that BatchNorm's backward
+        # reduction in its epilogue (stride 1, no channel padding, the NHWC buffers line up)
+        ctx.bn_src = None
+        if (bn_src is not None and BN_BWD_FUSION and need_dx and not want_skip and stride == (1, 1) and plan.cin_p == cin
+                and bn_src[0].shape == xin.shape):
+            ctx.bn_src = bn_src
+        ctx.wd_kmask = getattr(wd, "kmask", None)      # attributes do not survive save_for_backward
+        ctx.wf_kmask = getattr(wf, "kmask", None)      # wgrad skips tiles under all-zero mask blocks
+        # wgrad reads the activation as a logical NCHW tensor; the stem's im2col rows are 1x1 images of kp channels
+        ctx.save_for_backward(xin.view(-1, plan.wf_ld, 1, 1) if plan.stem else xin.permute(0, 3, 1, 2), m32, wd)
         ctx.desc = desc
         ctx.cin = cin
         ctx.has_bias = bias is not None
-        ctx.cout_p = cout_p
         ctx.x_dtype = x.dtype
         if want_skip:
             # second output = the input itself: whatever gradient reaches it (the identity path of a residual
@@ -1182,99 +1089,71 @@ class MaskedConv2dFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dy, *rest):
-        if getattr(ctx, "f32", False):
-            return _fp32_backward(ctx, dy)
         # outputs were (y [, x_skip] [, stats]); the statistics output is non-differentiable
         dskip = rest[0] if ctx.want_skip and rest else None
-        desc = ctx.desc
         if dy is None:          # only the skip output was used downstream
             return dskip, None, None, None, None, None, None, None, None, None, None
+        P, plan, desc = ctx.prec, ctx.plan, ctx.desc
         cout = desc.cout
         need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
         need_db = ctx.has_bias and ctx.needs_input_grad[3]
-        dyn = to_nhwc_bf16(dy, ctx.cout_p)
+        want_db = need_db and P.colsum_db
+        dyl = P.dy(dy, plan.cout_p)
+        x, m32, wd = ctx.saved_tensors
         dx = dw = db = None
         db_in_slot = False          # the bias gradient already sits in param.grad's arena slot: return None for it
-        if ctx.mode == "stem":
-            xg, m32 = ctx.saved_tensors
-            if need_dw:
-                r, s = desc.r, desc.s
-                cin = m32.shape[1]
-                ones = torch.ones(cout, xg.shape[1], dtype=torch.float32, device=xg.device)
-                gd = ctx.gdesc
-                dwm, db = conv_wgrad(gd, xg, dyn.view(-1, cout), ones.view(cout, -1, 1, 1), xg.shape[1], need_db)
-                # columns are (tap, channel group): back to OIHW and apply the mask (9.4 k elements)
-                cg = stem_geometry(cin, r, s)[0]
-                dw = dwm[:, :r * s * cg].reshape(cout, r * s, cg)[:, :, :cin].permute(0, 2, 1).reshape(cout, cin, r, s)
+        if need_dx:
+            addend = to_nhwc_bf16(dskip, ctx.cin) if dskip is not None else None
+            fused = None
+            if ctx.bn_src is not None and addend is None:
+                fused = conv_dgrad_bnrelu(ctx.xdesc, dyl, wd, ctx.bn_src, kmask=ctx.wd_kmask)
+            if fused is not None:
+                g, partial = fused
+                from . import fused_norm
+                fused_norm.offer_partials(g, partial, ctx.bn_src[5])          # picked up by that BatchNorm's backward
+                dx = g.permute(0, 3, 1, 2)
+            else:
+                # dX has the REAL channel count: the dgrad GEMM's N axis is cin, its K axis (taps x cout_p)
+                dx = P.dgrad(ctx.xdesc, dyl, wd, addend, ctx.wd_kmask).permute(0, 3, 1, 2)
+            if dx.dtype != ctx.x_dtype:
+                dx = dx.to(ctx.x_dtype)
+        if need_dw:
+            xa, dya = P.wgrad_operands(ctx.wdesc, x, dyl)
+            # dense: all-ones mask and no occupancy mask, so every tile of dW is computed
+            m, kmask = (_ones_like_mask(m32), None) if ctx.dense else (m32, ctx.wf_kmask)
+            if plan.stem:
+                # all kp columns (tap, channel) of the im2col GEMM: back to OIHW and apply the mask (9.4 k elements)
+                ones = torch.ones(cout, plan.wf_ld, 1, 1, dtype=torch.float32, device=m32.device)
+                dwm, db = P.wgrad(ctx.wdesc, xa, dya, ones, plan.wf_ld, want_db)
+                cin, r, s = m32.shape[1:]
+                dw = dwm[:, :r * s * cin].reshape(cout, r * s, cin).permute(0, 2, 1).reshape(cout, cin, r, s)
                 if not ctx.dense:
                     dw = dw * m32
-        else:
-            xn, m32, wd = ctx.saved_tensors
-            wf_kmask = ctx.wf_kmask
-            if ctx.dense:                      # all-ones mask and no occupancy mask: every tile of dW is computed
-                m32, wf_kmask = _ones_like_mask(m32), None
-            cin = ctx.cin                      # real input channels (desc.cin is the padded count the activation carries)
-            ddesc = desc
-            if ctx.cout_p != cout:
-                ddesc = _cabi.ConvDesc(desc.n, desc.h, desc.w, desc.cin, ctx.cout_p, desc.r, desc.s, desc.stride_h,
-                                       desc.stride_w, desc.pad_h, desc.pad_w, desc.p, desc.q)
-            if need_dx:
-                addend = None
-                if dskip is not None:
-                    addend = to_nhwc_bf16(dskip, cin)
-                # dX has the REAL channel count: the dgrad GEMM's N axis is cin, its K axis (taps x cout_p)
-                xdesc = ddesc if cin == desc.cin else _cabi.ConvDesc(desc.n, desc.h, desc.w, cin, ctx.cout_p, desc.r, desc.s,
-                                                                      desc.stride_h, desc.stride_w, desc.pad_h, desc.pad_w,
-                                                                      desc.p, desc.q)
-                fused = None
-                if ctx.bn_src is not None and addend is None:
-                    fused = conv_dgrad_bnrelu(xdesc, dyn, wd, ctx.bn_src, kmask=ctx.wd_kmask)
-                if fused is not None:
-                    g, partial = fused
-                    from . import fused_norm
-                    fused_norm.offer_partials(g, partial, ctx.bn_src[5])          # picked up by that BatchNorm's backward
-                    dx = g.permute(0, 3, 1, 2)
+            elif plan.cout_p != cout:
+                m_p = torch.zeros(plan.cout_p, *m.shape[1:], dtype=torch.float32, device=m.device)
+                m_p[:cout] = m
+                dwp, dbp = P.wgrad(ctx.wdesc, xa, dya, m_p, ctx.cin, want_db)
+                dw = dwp[:cout].contiguous()
+                db = dbp[:cout].contiguous() if dbp is not None else None
+            else:
+                ws_, bs_ = ctx.grad_slots if ctx.grad_slots is not None else (None, None)
+                dw_out = ws_ if ws_ is not None and ws_.is_contiguous() and ws_.numel() == m.numel() else None
+                db_out = bs_ if want_db else None
+
+                def run():
+                    out = P.wgrad(ctx.wdesc, xa, dya, m, ctx.cin, want_db, dw_out, db_out, kmask)
+                    grad_ready(dw_out, db_out)
+                    return out
+                if WGRAD_SIDE_STREAM and dw_out is not None and (db_out is not None or not want_db):
+                    dw, db = _on_wgrad_stream(run, xa, dya, m)   # nothing of it flows back through autograd
                 else:
-                    dx = conv_dgrad(xdesc, dyn, wd, addend, kmask=ctx.wd_kmask).permute(0, 3, 1, 2)
-                if dx.dtype != ctx.x_dtype:
-                    dx = dx.to(ctx.x_dtype)
-            if need_dw:
-                if ctx.cout_p != cout:
-                    m_p = torch.zeros(ctx.cout_p, *m32.shape[1:], dtype=torch.float32, device=m32.device)
-                    m_p[:cout] = m32
-                    dwp, dbp = conv_wgrad(ddesc, xn, dyn, m_p, cin, need_db)
-                    dw = dwp[:cout].contiguous()
-                    db = dbp[:cout].contiguous() if dbp is not None else None
-                else:
-                    ws_, bs_ = ctx.grad_slots if ctx.grad_slots is not None else (None, None)
-                    direct_w = ws_ is not None and ws_.is_contiguous() and ws_.numel() == m32.numel()
-                    direct_b = need_db and bs_ is not None
-                    if WGRAD_SIDE_STREAM and direct_w and (direct_b or not need_db):
-                        # nothing of this result flows back through autograd: run it beside the dgrad chain
-                        dev = xn.device
-                        cur, side = torch.cuda.current_stream(dev), _wgrad_stream(dev)
-                        ev = torch.cuda.Event(); ev.record(cur)
-                        side.wait_event(ev)
-                        with torch.cuda.stream(side):
-                            conv_wgrad(desc, xn, dyn, m32, cin, need_db, dw_out=ws_, db_out=bs_ if direct_b else None,
-                                       kmask=wf_kmask)
-                            grad_ready(ws_, bs_ if direct_b else None)
-                        _wgrad_keepalive.append((xn, dyn, m32))
-                        dw = db = None
-                        db_in_slot = direct_b
-                    else:
-                        dw, db = conv_wgrad(desc, xn, dyn, m32, cin, need_db, dw_out=ws_ if direct_w else None,
-                                            db_out=bs_ if direct_b else None, kmask=wf_kmask)
-                        if direct_w:
-                            dw = None
-                        if direct_b:
-                            db = None
-                            db_in_slot = True
-                        grad_ready(ws_ if direct_w else None, bs_ if direct_b else None)
+                    dw, db = run()
+                if dw_out is not None:
+                    dw = None
+                if db_out is not None:
+                    db, db_in_slot = None, True
         if need_db and db is None and not db_in_slot:
             db = dy.float().sum(dim=(0, 2, 3))
-        if dskip is not None and dx is None and need_dx is False:
-            dx = None
         return dx, dw, None, db, None, None, None, None, None, None, None
 
 
