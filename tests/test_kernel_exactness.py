@@ -511,6 +511,11 @@ def test_bn_backward_dgrad_epilogue_exact(dev, case):
       sum |g * xhat| and sum |g| of the channel; with dy >= 0, positive weights and a zero BatchNorm bias every term of a
       channel has one sign, and there the bar is relative to the value itself); the BatchNorm input gradient dy within
       2^-8 |reference| plus one bf16 ulp of the largest of its three terms k0 g, k1 y, k2, per element."""
+    bnb_dgrad_check(dev, case)
+
+
+def bnb_dgrad_check(dev, case):
+    """The checks of test_bn_backward_dgrad_epilogue_exact for one (id, n, hw, cin, cout, k) case."""
     from turboprune_b200 import ops
     lib = ops._cabi.load()
     name, n, hw, cin, cout, k = case

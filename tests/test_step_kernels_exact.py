@@ -336,9 +336,14 @@ def test_bn_forward_exact(dev, case):
       kernel's mean and the variance (the two-pass bar adds the variance error), num_batches_tracked + 1;
     - scale == fp32(w * invstd), shift == fp32(b - mean * scale) from save_mean / save_invstd, and z bit for bit."""
     from turboprune_b200 import _cabi
+    bn_forward_check(dev, case, _geom_checked(_cabi.load(), case))
+
+
+def bn_forward_check(dev, case, geom):
+    """The checks of test_bn_forward_exact for one BnCase whose bn_geom plan ``geom`` the caller has asserted."""
+    from turboprune_b200 import _cabi
     lib = _cabi.load()
     M, C = case.M, case.C
-    geom = _geom_checked(lib, case)
     g = torch.Generator(device=dev).manual_seed(M + C)
     y, _ = _bn_y(g, M, C, dev)
     res = _ints(g, (M, C), -8, 8, dev) if case.res else None
@@ -421,10 +426,15 @@ def test_bn_backward_exact(dev, case):
       exactly;
     - dy == bf16(fma(k0, g, fma(k1, y, k2))) from the kernel's coefficients, bit for bit (roundings as in _fma32)."""
     from turboprune_b200 import _cabi
+    bn_backward_check(dev, case, _geom_checked(_cabi.load(), case))
+
+
+def bn_backward_check(dev, case, geom):
+    """The checks of test_bn_backward_exact for one BnCase whose bn_geom plan ``geom`` the caller has asserted."""
+    from turboprune_b200 import _cabi
     lib = _cabi.load()
     M, C = case.M, case.C
     relu, want_dres = BWD_MODES[case.bwd]
-    geom = _geom_checked(lib, case)
     g_ = torch.Generator(device=dev).manual_seed(M + C + 1)
     y, ymax = _bn_y(g_, M, C, dev)
     pick = lambda vals: torch.tensor(vals, device=dev)[torch.randint(0, len(vals), (C,), generator=g_, device=dev)]
