@@ -375,6 +375,64 @@ int tp_adamw(void* const* w, const void* const* g, void* const* exp_avg, void* c
              const int64_t* numel, int n_seg, const float* inv_lr_dev, const float* decay_dev,
              double beta1, double beta2, double eps, int table_cached, void* ws, size_t ws_bytes, void* stream);
 
+/* ---- Muon (optimizer_name: MuonAdamW) ----------------------------------------------------
+ * torch.optim.Muon for every hidden masked layer of a model at once, on the 2-D view [a][b] = p.view(p.shape[0], -1)
+ * of each weight.  Per layer, with u the nesterov (or plain) momentum and X = bf16(u), transposed when a > b:
+ *   buf = lerp(buf, g, 1 - mu);  u = nesterov ? lerp(g, buf, mu) : buf;  X /= clamp(|X|_F, eps);
+ *   ns_steps times: G = X X^T;  H = b G + c G G;  X = a X + H X       (bf16 operands, fp32 accumulation)
+ *   w = w * fp32(1 - lr wd);  w = w + fp32(-lr ratio) * O            (O = X, transposed back)
+ * The reference's config schema names Muon (utils/harness_params.py:63) but its harness builds SGD for it; the name
+ * MuonAdamW trains Muon for the hidden weights and AdamW (tp_adamw) for every other parameter.
+ *
+ * Workspace: one bf16 buffer of 64-element rows (128 B).  A matrix [mp][np] (both multiples of 64) is stored in PANEL
+ * layout: element (i, j) at row base + (j / 64) * mp + i, column j % 64, so every 64 x 64 tile is 8 KB of contiguous
+ * rows and one 2-D TMA map with a 64 x 64 box covers every matrix of every layer.  Per layer the caller places X's two
+ * buffers (x0, x1: mp = min(a, b), np = max(a, b), both padded up to 64) and G, H ([mp][mp]).  Padding rows and columns
+ * are zero and stay exactly zero through the iterations.  Layers are numbered in 64 x 64 X tiles: layer l owns tiles
+ * tile0 .. tile0 + (mp / 64) * (np / 64) - 1 of the elementwise launches, row-major over (mp / 64, np / 64). */
+typedef struct tp_muon_layer {
+  void* w; const void* g; void* buf;   /* fp32 [a][b] contiguous: weight, gradient, momentum_buffer */
+  int32_t a, b;                        /* the 2-D view's shape */
+  int32_t trans;                       /* 1: X = U^T (a > b) */
+  int32_t mp, np;                      /* X extents, multiples of 64 */
+  int32_t tile0;                       /* first 64 x 64 X tile of this layer */
+  int64_t x0, x1;                      /* workspace rows of X's two buffers */
+  double ratio;                        /* torch's _adjust_lr factor of the 2-D shape: the step's lr is lr * ratio */
+} tp_muon_layer;
+/* Bytes of `table_ws` for tp_muon_prepare / tp_muon_normalize / tp_muon_apply: the layer table and one completion count
+ * per layer. */
+size_t tp_muon_workspace_bytes(int n_layers);
+/* The momentum lerps, bf16(u) into x0 (transposed where trans, zero padding), one fp32 sum of squares of the bf16 values
+ * per X tile into partial[n_tiles], and per layer norms[l] = bf16(sqrt(sum of the layer's partials, folded in a fixed
+ * order)), clamped below at eps in fp32 and rounded to bf16 again (ortho_grad.norm().clamp(min=eps)).  The fold runs
+ * once per layer, in the CTA that finishes the layer's last tile (an integer completion count, restarted by that CTA).
+ * One launch over all n_tiles tiles.  momentum: the Python float (1 - mu is formed in double, then fp32, as ATen does).
+ * norms: DEVICE fp32 [n_layers].  table_cached != 0: `table_ws` still holds the table of an earlier call with identical
+ * layers, no host->device copy (capturable); layers may then be NULL. */
+int tp_muon_prepare(const tp_muon_layer* layers, int n_layers, int64_t n_tiles, int table_cached, void* xws,
+                    void* partial, void* norms, double momentum, int nesterov, double eps, void* table_ws,
+                    size_t table_bytes, void* stream);
+/* x0 = bf16(x0 / norms[l]) in place (ATen's bf16 div_).  One launch; table_ws as left by tp_muon_prepare. */
+int tp_muon_normalize(int n_layers, int64_t n_tiles, void* xws, const void* norms, const void* table_ws, void* stream);
+/* One GEMM of a Newton-Schulz step for every layer at once: out = bf16(alpha * acc + beta * C) over a tile list.
+ *   mode 0 GRAM   G = X X^T          both operands K-major (rows of X)
+ *   mode 1 POLY   H = c G G + b G    both operands K-major (G is exactly symmetric)
+ *   mode 2 UPDATE X' = H X + a X     B MN-major (64 K rows of X in one panel)
+ * tiles: DEVICE int32 [n_tiles][8] = {a0, b0, sa, sb, nk, c0, o0, m0}: output tile (64 x 64) = sum over nk K blocks of
+ * A rows a0 + k sa times B rows b0 + k sb (64 x 64 boxes); C (c0 >= 0) the 64 rows at c0; the result goes to the rows at
+ * o0 and, transposed, to the rows at m0 (m0 >= 0; m0 == o0: a diagonal tile, made exactly symmetric from its upper
+ * triangle).  GRAM and POLY compute upper tiles only and mirror them, so G and H are exactly symmetric.  A persistent,
+ * warp-specialised wgmma + TMA kernel (one producer warp, one consumer warpgroup per CTA, several CTAs per SM) walks the
+ * list in order: sort it longest K first.  No atomics, no split-K: deterministic.  ws_rows: rows of the workspace. */
+int tp_muon_ns_gemm(int mode, void* xws, int64_t ws_rows, const void* tiles, int n_tiles, float alpha, float beta,
+                    void* stream);
+/* w = w * fp32(1 - lr wd); w = w + fp32(-(lr ratio_l)) * O  (one FMA, as ATen's add_(alpha=) contracts it), O = the X
+ * buffer `which` (0: x0, 1: x1) transposed back.  lr_wd: DEVICE double [2] = (lr, weight_decay); both factors are formed
+ * with correctly rounded double ops, as Python forms them, so a captured step follows the LR schedule.  One launch;
+ * table_ws as left by tp_muon_prepare. */
+int tp_muon_apply(int n_layers, int64_t n_tiles, const void* xws, int which, const void* lr_wd, const void* table_ws,
+                  void* stream);
+
 /* ---- gradient exchange over NVLink/NVSwitch peer memory ---------------------------------
  * Replaces the c10d Reducer's per-bucket  grad/W -> ncclAllReduce(SUM) -> copy back
  * (harness_definitions/base_harness.py:81) with one kernel: every rank reads its peers'

@@ -27,6 +27,12 @@ class StageItem(ctypes.Structure):
                [("kmask_f", c_void_p), ("kmask_d", c_void_p)]
 
 
+class MuonLayer(ctypes.Structure):
+    _fields_ = [("w", c_void_p), ("g", c_void_p), ("buf", c_void_p)] + \
+               [(n, c_int32) for n in ("a", "b", "trans", "mp", "np", "tile0")] + [("x0", c_int64), ("x1", c_int64),
+                                                                                  ("ratio", c_double)]
+
+
 class CropEntry(ctypes.Structure):
     _fields_ = [("src", c_void_p)] + [(n, c_int32) for n in ("H", "W", "top", "left", "h", "w", "flip", "reserved")]
 
@@ -110,6 +116,13 @@ SIGNATURES = {
     "tp_stage_weights_batched_f32": (c_int, [POINTER(StageItem), c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "tp_to_nhwc_f32": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int64, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     "tp_im2col_stem_f32": (c_int, [c_void_p, c_int64, c_int64, c_int64, c_int64] + [c_int] * 13 + [c_void_p, c_int, c_void_p]),
+    # Muon
+    "tp_muon_workspace_bytes": (c_size_t, [c_int]),
+    "tp_muon_prepare": (c_int, [POINTER(MuonLayer), c_int, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_double, c_int,
+                                c_double, c_void_p, c_size_t, c_void_p]),
+    "tp_muon_normalize": (c_int, [c_int, c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "tp_muon_ns_gemm": (c_int, [c_int, c_void_p, c_int64, c_void_p, c_int, c_float, c_float, c_void_p]),
+    "tp_muon_apply": (c_int, [c_int, c_int64, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
 }
 
 

@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIBNAME = "libturboprune_b200.so"
-SOURCES = ["tp_core.cu", "tp_prune.cu", "tp_optim.cu", "tp_igemm.cu", "tp_reduce.cu", "tp_bn.cu", "tp_pool.cu", "tp_data.cu"]
+SOURCES = ["tp_core.cu", "tp_prune.cu", "tp_optim.cu", "tp_igemm.cu", "tp_reduce.cu", "tp_bn.cu", "tp_pool.cu", "tp_data.cu", "tp_muon.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-cudart", "static",

@@ -52,6 +52,13 @@ inline cudaError_t launch(void (*kernel)(KA...), dim3 grid, dim3 block, size_t s
   cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KA>(args)...);
 }
+
+// ATen's fp32 lerp(self, end, weight) with a scalar weight (two branches on |weight| < 0.5; omw = 1 - weight in fp32):
+// nvcc contracts `self + weight * (end - self)` into one FMA, as the torch build does.  AdamW's exp_avg update and
+// Muon's momentum and nesterov lerps.
+__device__ __forceinline__ float adamw_lerp(float m, float g, float wt, float omw, bool small) {
+  return small ? fmaf(wt, __fsub_rn(g, m), m) : fmaf(-__fsub_rn(g, m), omw, g);
+}
 #endif
 
 // A bump allocator over the caller's workspace.

@@ -999,6 +999,12 @@ static int make_tiled_map(CUtensorMap* m, const void* ptr, uint64_t cols, uint64
   return TP_OK;
 }
 
+// The same map for callers in other translation units (tp_muon.cu's workspace), with the driver entry points loaded.
+int make_tiled_map_bf16(CUtensorMap* m, const void* ptr, uint64_t cols, uint64_t rows, uint64_t ld_elems, uint32_t box_rows) {
+  int rc = load_driver_fns(); if (rc) return rc;
+  return make_tiled_map(m, ptr, cols, rows, ld_elems, box_rows);
+}
+
 // im2col map over NHWC bf16 [n][h][w][c]: `pixels` consecutive iteration positions x 64 channels.
 // Iteration grid (P_it x Q_it per image) starts at (base_h, base_w) and advances by (step_h, step_w).
 // f32: NHWC fp32, 32 channels per pixel row (128 B).

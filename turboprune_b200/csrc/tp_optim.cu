@@ -488,10 +488,7 @@ __global__ void __launch_bounds__(256) k_sgd(const Seg* __restrict__ segs, int n
 //   d = (sqrt(v) / b + eps) / s              IEEE ops, no contraction possible
 //   _foreach_addcdiv_(w, m, d)               w + m / d                      alpha == 1: no FMA
 // Settled on an H100 against torch 2.11 / CUDA 12.8 (tests/test_adamw.py compares every bit of w, m, v and step; powf
-// matched ATen's for every t in 1..300 and 10001..10059).
-__device__ __forceinline__ float adamw_lerp(float m, float g, float wt, float omw, bool small) {
-  return small ? fmaf(wt, __fsub_rn(g, m), m) : fmaf(-__fsub_rn(g, m), omw, g);
-}
+// matched ATen's for every t in 1..300 and 10001..10059).  The lerp is adamw_lerp (tp_common.cuh).
 
 struct AdamWCoef { float c, w1, omw1, b2, w2, eps, s, b; bool decay, small; };
 

@@ -4,7 +4,8 @@
 reference's behaviour (:28-50, :159-269): a fresh optimizer and LR schedule per level (momentum never carries
 over), ``model_init.pt`` / ``optimizer_init.pt`` at level 0, ``model_rewind.pt`` at ``pruning_params.rewind_epoch``,
 per-level CSV + summary CSV.  Optimizer = ``FusedSGD`` (same state-dict layout as torch.optim.SGD), or ``FusedAdamW``
-(torch.optim.AdamW's) when ``optimizer_params.optimizer_name`` is ``AdamW``.  Loaders: the
+(torch.optim.AdamW's) when ``optimizer_params.optimizer_name`` is ``AdamW``, or ``FusedMuon`` (Muon for the hidden masked
+weights, AdamW for the rest) when it is ``MuonAdamW``.  Loaders: the
 reference's device-resident CIFAR loader (``AirbenchLoaders``) when a CIFAR config names a ``dataset_params.dataloader_type``
 other than ``synthetic`` (the reference's ``dp_cifar*.yaml`` say ``torch``); ``ImageFolderImagenet`` (GPU-decoded
 ImageFolder tree) when an ImageNet config says ``dataloader_type: imagefolder``; otherwise (FFCV / WebDataset are out of
@@ -24,7 +25,7 @@ import torch
 import torch.nn as nn
 from torch.amp import autocast
 
-from ..optim import FusedAdamW, FusedSGD
+from ..optim import FusedAdamW, FusedMuon, FusedSGD
 from ..utils import schedulers
 from ..utils.custom_models import CustomModel, TorchVisionModel
 from ..utils.dataset import AirbenchLoaders, ImageFolderImagenet, SyntheticLoaders
@@ -82,9 +83,35 @@ class PruningHarness(BaseHarness):
             self.optimizer = FusedAdamW(self.model.parameters(), lr=o.lr, betas=tuple(o.get("betas") or (0.9, 0.999)),
                                         eps=o.get("eps") or 1e-8, weight_decay=o.weight_decay, capturable=True)
             return
-        # SGD, and (as in the reference, whose harness builds SGD whatever the name says) every other name
+        if o.get("optimizer_name", "SGD") == "MuonAdamW":
+            self.optimizer = self._muon_adamw(o)
+            return
+        # SGD, and (as in the reference, whose harness builds SGD whatever the name says) every other name (Muon too)
         self.optimizer = FusedSGD(self.model.parameters(), lr=o.lr, momentum=o.momentum, weight_decay=o.weight_decay,
                                   capturable=True)
+
+    def _muon_adamw(self, o):
+        """Muon for the weights of every masked layer but the classifier (the last masked layer in module order, whose
+        output width is the class count), AdamW for every other parameter: biases, norms, the classifier, DeiT's
+        unmasked patch embedding.  One lr and one weight decay serve both groups: ``adjust_lr_fn`` defaults to
+        ``match_rms_adamw``, which scales Muon's step to AdamW's update RMS."""
+        from ..utils.mask_layers import MASKED_LAYER_TYPES
+        masked = [m for m in self.model.modules() if isinstance(m, MASKED_LAYER_TYPES)]
+        if not masked:
+            raise ValueError("MuonAdamW: the model has no masked layer to train with Muon")
+        head = masked[-1]
+        num_classes = getattr(self, "num_classes", None)
+        assert num_classes is None or head.weight.shape[0] == num_classes, \
+            f"MuonAdamW: the last masked layer has {head.weight.shape[0]} outputs, not the {num_classes} classes"
+        hidden = [m.weight for m in masked[:-1]]
+        ids = {id(w) for w in hidden}
+        rest = [p for p in self.model.parameters() if id(p) not in ids]
+        groups = [dict(params=hidden, use_muon=True), dict(params=rest, use_muon=False)]
+        return FusedMuon([g for g in groups if g["params"]], lr=o.lr, weight_decay=o.weight_decay, momentum=o.momentum,
+                         nesterov=bool(o.get("nesterov", True)), ns_steps=int(o.get("ns_steps", 5)),
+                         adjust_lr_fn=o.get("adjust_lr_fn", "match_rms_adamw"),
+                         adamw_betas=tuple(o.get("betas") or (0.9, 0.999)), adamw_eps=o.get("eps") or 1e-8,
+                         capturable=True)
 
     def _setup_scheduler(self, epochs_per_level):
         kind = self.cfg.optimizer_params.scheduler_type

@@ -3,11 +3,13 @@ arithmetic is ours).  Every function here launches hand-written sm_90a kernels t
 ``_cabi`` — there is no eager / CPU fallback.
 """
 import ctypes
+import math
 import threading
 from contextlib import contextmanager
 from ctypes import c_void_p
 from typing import Callable, NamedTuple, Optional
 
+import numpy as np
 import torch
 
 from . import _cabi
@@ -454,6 +456,136 @@ def adamw_step(params, grads, exp_avgs, exp_avg_sqs, steps, inv_lr_dev, decay_de
                           wsb.numel(), _cabi.stream_ptr(dev))
     _cabi.check(rc, "tp_adamw")
     _count(2)
+
+
+MUON_GRAM, MUON_POLY, MUON_UPDATE = 0, 1, 2
+
+
+def _pad64(v):
+    return (v + 63) // 64 * 64
+
+
+def muon_ratio(a, b, adjust_lr_fn):
+    """torch.optim.Muon's ``_adjust_lr`` factor for the 2-D shape [a, b] (``lr * ratio`` is the step's lr)."""
+    if adjust_lr_fn is None or adjust_lr_fn == "original":
+        return math.sqrt(max(1, a / b))
+    if adjust_lr_fn == "match_rms_adamw":
+        return 0.2 * math.sqrt(max(a, b))
+    return 1.0
+
+
+class MuonPlan:
+    """Workspace layout and tile lists of one Muon step over layers of 2-D shapes ``shapes`` = [(a, b), ...].
+
+    Layer l: X = U (a <= b) or U^T (a > b), [mp][np] = (min, max) padded up to 64, in the panel layout of
+    include/turboprune_b200.h; its rows x0 / x1 (the ping-pong pair), g (G = X X^T) and h (H) follow one another in one
+    bf16 workspace of ``rows`` x 64.  ``n_tiles`` 64 x 64 X tiles drive the elementwise launches (layer l from
+    ``tile0[l]``).  ``gemm_tiles[(mode, src)]``: int32 [n, 8] tile list of a Newton-Schulz GEMM reading X buffer src (0
+    or 1), longest K first; UPDATE writes buffer 1 - src."""
+
+    def __init__(self, shapes):
+        self.shapes = [(int(a), int(b)) for a, b in shapes]
+        self.trans, self.mp, self.np, self.tile0, self.x = [], [], [], [], []
+        self.g, self.h = [], []
+        rows = tiles = 0
+        for a, b in self.shapes:
+            mp, np_ = _pad64(min(a, b)), _pad64(max(a, b))
+            self.trans.append(a > b)
+            self.mp.append(mp)
+            self.np.append(np_)
+            self.tile0.append(tiles)
+            tiles += (mp // 64) * (np_ // 64)
+            xr, gr = mp * np_ // 64, mp * mp // 64
+            self.x.append((rows, rows + xr))
+            self.g.append(rows + 2 * xr)
+            self.h.append(rows + 2 * xr + gr)
+            rows += 2 * xr + 2 * gr
+        self.rows, self.n_tiles = rows, tiles
+        self.gemm_tiles = {}
+        for src in (0, 1):
+            for mode in (MUON_GRAM, MUON_POLY, MUON_UPDATE):
+                if mode == MUON_POLY and src == 1:
+                    continue
+                self.gemm_tiles[(mode, src)] = self._tiles(mode, src)
+
+    def _tiles(self, mode, src):
+        out = []
+        for l in range(len(self.shapes)):
+            mp, np_, g, h = self.mp[l], self.np[l], self.g[l], self.h[l]
+            x, xo = self.x[l][src], self.x[l][1 - src]
+            tm, tn = mp // 64, np_ // 64
+            if mode == MUON_UPDATE:                  # X' = H X + a X: A = rows of H, B = 64 K rows of X's panel tn
+                out += [(h + ti * 64, x + t * mp, mp, 64, tm, x + t * mp + ti * 64, xo + t * mp + ti * 64, -1)
+                        for ti in range(tm) for t in range(tn)]
+                continue
+            src_rows, nk, dst = (x, tn, g) if mode == MUON_GRAM else (g, tm, h)
+            for ti in range(tm):
+                for tk in range(ti, tm):                 # upper tiles; each is mirrored into (tk, ti)
+                    c0 = g + tk * mp + ti * 64 if mode == MUON_POLY else -1
+                    out.append((src_rows + ti * 64, src_rows + tk * 64, mp, mp, nk, c0,
+                                dst + tk * mp + ti * 64, dst + ti * mp + tk * 64))
+        out.sort(key=lambda t: -t[4])                    # longest K first (stable)
+        return np.asarray(out, dtype=np.int32).reshape(-1, 8)
+
+    def ratios(self, adjust_lr_fn):
+        return [muon_ratio(a, b, adjust_lr_fn) for a, b in self.shapes]
+
+    def layer_table(self, ws, gs, bufs, adjust_lr_fn):
+        """ctypes array of tp_muon_layer for the fp32 [a][b] weights / gradients / momentum buffers."""
+        arr = (_cabi.MuonLayer * len(self.shapes))()
+        for l, ((a, b), r) in enumerate(zip(self.shapes, self.ratios(adjust_lr_fn))):
+            arr[l] = _cabi.MuonLayer(ws[l].data_ptr(), gs[l].data_ptr(), bufs[l].data_ptr(), a, b, int(self.trans[l]),
+                                     self.mp[l], self.np[l], self.tile0[l], self.x[l][0], self.x[l][1], r)
+        return arr
+
+
+def muon_prepare(plan, xws, partial, norms, table_ws, ws, gs, bufs, momentum, nesterov, eps, adjust_lr_fn,
+                 table_cached=False):
+    """Momentum lerps, bf16(u) into X buffer 0, per-tile sums of squares and each layer's clamped bf16 norm into the fp32
+    device tensor ``norms`` (one launch).  ``ws`` / ``gs`` / ``bufs``: contiguous fp32 [a][b] views; with
+    ``table_cached`` they are not read (the table in ``table_ws``, which carries each layer's lr ratio, is reused)."""
+    lib = _cabi.load()
+    dev = xws.device
+    layers = None if table_cached else plan.layer_table(ws, gs, bufs, adjust_lr_fn)
+    with torch.cuda.device(dev):
+        rc = lib.tp_muon_prepare(layers, len(plan.shapes), plan.n_tiles, int(bool(table_cached)), c_void_p(xws.data_ptr()),
+                                 c_void_p(partial.data_ptr()), c_void_p(norms.data_ptr()), float(momentum),
+                                 int(bool(nesterov)), float(eps), c_void_p(table_ws.data_ptr()), table_ws.numel(),
+                                 _cabi.stream_ptr(dev))
+    _cabi.check(rc, "tp_muon_prepare")
+    _count()
+
+
+def muon_normalize(plan, xws, norms, table_ws):
+    lib = _cabi.load()
+    dev = xws.device
+    with torch.cuda.device(dev):
+        rc = lib.tp_muon_normalize(len(plan.shapes), plan.n_tiles, c_void_p(xws.data_ptr()), c_void_p(norms.data_ptr()),
+                                   c_void_p(table_ws.data_ptr()), _cabi.stream_ptr(dev))
+    _cabi.check(rc, "tp_muon_normalize")
+    _count()
+
+
+def muon_ns_gemm(mode, xws, tiles_dev, alpha, beta):
+    """One Newton-Schulz GEMM over the int32 [n, 8] device tile list ``tiles_dev`` (see tp_muon_ns_gemm)."""
+    lib = _cabi.load()
+    dev = xws.device
+    with torch.cuda.device(dev):
+        rc = lib.tp_muon_ns_gemm(int(mode), c_void_p(xws.data_ptr()), xws.numel() // 64, c_void_p(tiles_dev.data_ptr()),
+                                 tiles_dev.shape[0], float(alpha), float(beta), _cabi.stream_ptr(dev))
+    _cabi.check(rc, "tp_muon_ns_gemm")
+    _count()
+
+
+def muon_apply(plan, xws, which, lr_wd, table_ws):
+    """w = w * fp32(1 - lr wd) + fp32(-(lr ratio)) * O; ``lr_wd``: float64 device tensor (lr, weight_decay)."""
+    lib = _cabi.load()
+    dev = xws.device
+    with torch.cuda.device(dev):
+        rc = lib.tp_muon_apply(len(plan.shapes), plan.n_tiles, c_void_p(xws.data_ptr()), int(which),
+                               c_void_p(lr_wd.data_ptr()), c_void_p(table_ws.data_ptr()), _cabi.stream_ptr(dev))
+    _cabi.check(rc, "tp_muon_apply")
+    _count()
 
 
 # ---------------------------------------------------------------------------------------------
