@@ -374,6 +374,24 @@ size_t tp_segtable_workspace_bytes(int n_seg);
 int tp_adamw(void* const* w, const void* const* g, void* const* exp_avg, void* const* exp_avg_sq, void* const* step,
              const int64_t* numel, int n_seg, const float* inv_lr_dev, const float* decay_dev,
              double beta1, double beta2, double eps, int table_cached, void* ws, size_t ws_bytes, void* stream);
+/* Schedule-Free SGD (the schedulefree package's SGDScheduleFree, foreach branch; optimizer_params.scheduler_type:
+ * ScheduleFree), one launch for all segments, bit for bit with the package's torch ops:
+ *   g' = g + wd y (wd != 0);  y = lerp(y, z, ckp1);  y += alpha_y g';  z -= lr g'
+ * g' is not written back to g.
+ *   y, g, z      : HOST arrays of n_seg DEVICE pointers (fp32, contiguous): parameter, gradient, the state `z`
+ *   scalars_dev  : DEVICE float [3] = (lr, ckp1, alpha_y = lr (momentum (1 - ckp1) - 1)), each formed in double and
+ *                  rounded to fp32; the host refreshes it every step, so a captured step follows the schedule
+ *   weight_decay : the Python float (rounded to fp32 in here; no decay term at all when it is 0)
+ *   first_step   : z does not exist yet: it starts as a copy of y (the package's clone(p)) inside this launch
+ * 20 B/elem.  table_cached: as tp_sgd_momentum (capturable).  Workspace: tp_segtable_workspace_bytes(n_seg). */
+int tp_schedulefree_sgd(void* const* y, const void* const* g, void* const* z, const int64_t* numel, int n_seg,
+                        const float* scalars_dev, double weight_decay, int first_step, int table_cached,
+                        void* ws, size_t ws_bytes, void* stream);
+/* y = lerp(y, z, fp32(weight)) for all segments, bit for bit with torch's per-tensor Tensor.lerp_(z, weight): the
+ * schedule-free eval() (weight 1 - 1 / momentum: y -> x) and train() (weight 1 - momentum: x -> y).  12 B/elem, one
+ * launch.  table_cached and workspace: as tp_schedulefree_sgd. */
+int tp_schedulefree_swap(void* const* y, const void* const* z, const int64_t* numel, int n_seg, double weight,
+                         int table_cached, void* ws, size_t ws_bytes, void* stream);
 
 /* ---- Muon (optimizer_name: MuonAdamW) ----------------------------------------------------
  * torch.optim.Muon for every hidden masked layer of a model at once, on the 2-D view [a][b] = p.view(p.shape[0], -1)

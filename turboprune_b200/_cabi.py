@@ -93,6 +93,10 @@ SIGNATURES = {
                          c_size_t, c_void_p]),
     "tp_rigl_apply_states": (c_int, [POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), c_int,
                                      POINTER(c_int64), c_int, c_void_p, c_size_t, c_void_p]),
+    "tp_schedulefree_sgd": (c_int, [POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), POINTER(c_int64), c_int,
+                                    c_void_p, c_double, c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    "tp_schedulefree_swap": (c_int, [POINTER(c_void_p), POINTER(c_void_p), POINTER(c_int64), c_int, c_double, c_int,
+                                     c_void_p, c_size_t, c_void_p]),
     "tp_p2p_allreduce_mask": (c_int, [POINTER(c_void_p), POINTER(c_void_p), c_int, c_int, c_int64, c_void_p, c_float,
                                       c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "tp_bn_workspace_bytes": (c_size_t, [c_int64, c_int]),

@@ -557,6 +557,111 @@ __global__ void __launch_bounds__(256) k_adamw(const Seg* __restrict__ segs, int
   }
 }
 
+// Schedule-Free SGD (Defazio et al. 2024; the schedulefree package's SGDScheduleFree, foreach branch): one launch for all
+// parameters.  20 B/elem: read y, g, z; write y, z (the four torch launches move 48 B/elem, 36 without weight decay).
+// The segment table is SGD's with these roles: w = y (the parameter), g = gradient, buf = z.  Per element, the ops ATen
+// runs, in the same order and rounding (opmath fp32; lr, ckp1 and alpha_y = lr * (momentum * (1 - ckp1) - 1) are Python
+// doubles rounded to fp32, as Scalar.to<float>() does):
+//   _foreach_add_(g, y, alpha=wd)        g' = fma(wd, y, g)             only when wd != 0 (as in k_sgd)
+//   _foreach_lerp_(y, z, weight=ckp1)    ATen's two-branch lerp (adamw_lerp, tp_common.cuh)
+//   _foreach_add_(y, g', alpha=alpha_y)  fma(alpha_y, g', y)            ATen's `a + alpha * b`, contracted by nvcc
+//   _foreach_sub_(z, g', alpha=lr)       fma(-lr, g', z)                ATen's `a - alpha * b`, contracted the same way
+// Settled on an H100 against torch 2.11 / CUDA 12.8: tests/test_schedulefree.py compares every bit of y and z with the
+// torch sequence over ResNet-50's and DeiT-S's parameters, with and without weight decay, through the warm-up.
+// The package also writes g' back into the gradient; nothing reads p.grad after the step (the gradient storage is zeroed
+// before the next backward), so this kernel does not.  first != 0: z does not exist yet and starts as a copy of y
+// (the package's clone(p)), made here instead of in a launch of its own.
+struct SFCoef { float lr, ckp1, omc, ay, wd; bool decay, small; };
+
+__device__ __forceinline__ void schedulefree_elem(float& y, float g, float& z, const SFCoef& k) {
+  const float gd = k.decay ? fmaf(k.wd, y, g) : g;
+  y = fmaf(k.ay, gd, adamw_lerp(y, z, k.ckp1, k.omc, k.small));
+  z = fmaf(-k.lr, gd, z);
+}
+
+__global__ void __launch_bounds__(256) k_schedulefree(const Seg* __restrict__ segs, int n_seg, long long tiles,
+                                                      const float* __restrict__ sc, float wd, int decay, int first) {
+  pdl_enter();
+  SFCoef k;
+  k.lr = sc[0]; k.ckp1 = sc[1]; k.ay = sc[2]; k.wd = wd; k.decay = decay != 0;
+  k.omc = __fsub_rn(1.f, k.ckp1); k.small = fabsf(k.ckp1) < 0.5f;
+  const int t = threadIdx.x;
+  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const Seg sg = segs[find_seg(segs, n_seg, tile)];
+    const long long base = (tile - sg.tile0) * kTileElems;
+    const long long rem = sg.n - base;
+    const int n_in = rem < kTileElems ? (int)rem : kTileElems;
+    float* yp = const_cast<float*>(sg.w) + base;
+    const float* gp = sg.g + base;
+    float* zp = sg.buf + base;
+    const bool vec = n_in == kTileElems && ((((uintptr_t)yp) | ((uintptr_t)gp) | ((uintptr_t)zp)) & 15) == 0;
+    if (vec) {
+#pragma unroll
+      for (int it = 0; it < kTileElems / (256 * 4); ++it) {
+        const int q = it * 256 + t;
+        float4 y = ((const float4*)yp)[q];
+        const float4 g = ld_stream((const float4*)gp + q);
+        float4 z = first ? y : ((const float4*)zp)[q];
+        schedulefree_elem(y.x, g.x, z.x, k); schedulefree_elem(y.y, g.y, z.y, k);
+        schedulefree_elem(y.z, g.z, z.z, k); schedulefree_elem(y.w, g.w, z.w, k);
+        ((float4*)zp)[q] = z;
+        ((float4*)yp)[q] = y;
+      }
+    } else {
+      for (int i = t; i < n_in; i += 256) {
+        float y = yp[i], z = first ? yp[i] : zp[i];
+        schedulefree_elem(y, gp[i], z, k);
+        zp[i] = z; yp[i] = y;
+      }
+    }
+  }
+}
+
+// y = lerp(y, z, w) for every segment (w = y, buf = z): torch's per-tensor Tensor.lerp_(z, w) with a Python-scalar weight,
+// the schedule-free train() / eval() switch.  12 B/elem.
+__global__ void __launch_bounds__(256) k_lerp_segs(const Seg* __restrict__ segs, int n_seg, long long tiles, float wt) {
+  pdl_enter();
+  const float omw = __fsub_rn(1.f, wt);
+  const bool small = fabsf(wt) < 0.5f;
+  const int t = threadIdx.x;
+  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const Seg sg = segs[find_seg(segs, n_seg, tile)];
+    const long long base = (tile - sg.tile0) * kTileElems;
+    const long long rem = sg.n - base;
+    const int n_in = rem < kTileElems ? (int)rem : kTileElems;
+    float* yp = const_cast<float*>(sg.w) + base;
+    const float* zp = sg.buf + base;
+    if (n_in == kTileElems && ((((uintptr_t)yp) | ((uintptr_t)zp)) & 15) == 0) {
+#pragma unroll
+      for (int it = 0; it < kTileElems / (256 * 4); ++it) {
+        const int q = it * 256 + t;
+        float4 y = ((const float4*)yp)[q];
+        const float4 z = ld_stream((const float4*)zp + q);
+        y.x = adamw_lerp(y.x, z.x, wt, omw, small); y.y = adamw_lerp(y.y, z.y, wt, omw, small);
+        y.z = adamw_lerp(y.z, z.z, wt, omw, small); y.w = adamw_lerp(y.w, z.w, wt, omw, small);
+        ((float4*)yp)[q] = y;
+      }
+    } else {
+      for (int i = t; i < n_in; i += 256) yp[i] = adamw_lerp(yp[i], zp[i], wt, omw, small);
+    }
+  }
+}
+
+// The segment table of an optimizer launch: uploaded, or (table_cached) the one an earlier call with the same pointers
+// left in `ws`, in which case only the tiles are counted and no host->device copy is issued (capturable).
+static int seg_table(Arena& ar, int table_cached, void* const* w, const void* const* g, void* const* buf,
+                     const int64_t* numel, int n_seg, Seg** d_segs, long long* tiles, cudaStream_t st) {
+  *tiles = 0;
+  if (!table_cached) return upload_segs(ar, (const void* const*)w, g, nullptr, nullptr, buf, numel, n_seg, d_segs, tiles, nullptr, st);
+  *d_segs = (Seg*)ar.take(sizeof(Seg) * n_seg);
+  if (!*d_segs) return TP_ERR_WORKSPACE;
+  for (int i = 0; i < n_seg; ++i) {
+    if (numel[i] < 0) return TP_ERR_INVALID;
+    *tiles += (numel[i] + kTileElems - 1) / kTileElems;
+  }
+  return TP_OK;
+}
+
 }  // namespace tp
 
 using namespace tp;
@@ -831,6 +936,40 @@ int tp_adamw(void* const* w, const void* const* g, void* const* exp_avg, void* c
     launch(k_adamw, (unsigned)(tiles < gmax ? tiles : gmax), 256, 0, st, (const Seg*)d_segs, n_seg, tiles, inv_lr_dev, decay_dev,
            (float)beta1, (float)beta2, (float)(1.0 - beta1), (float)(1.0 - beta2), (float)eps);
   }
+  TP_LAUNCH_CHECK();
+  return TP_OK;
+}
+
+int tp_schedulefree_sgd(void* const* y, const void* const* g, void* const* z, const int64_t* numel, int n_seg,
+                        const float* scalars_dev, double weight_decay, int first_step, int table_cached,
+                        void* ws, size_t ws_bytes, void* stream) {
+  if (!numel || n_seg <= 0 || !scalars_dev || !ws) return TP_ERR_INVALID;
+  if (!table_cached && (!y || !g || !z)) return TP_ERR_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  Arena ar(ws, ws_bytes);
+  Seg* d_segs = nullptr; long long tiles = 0;
+  int rc = seg_table(ar, table_cached, y, g, z, numel, n_seg, &d_segs, &tiles, st);
+  if (rc) return rc;
+  if (tiles == 0) return TP_OK;
+  const long long gmax = (long long)sm_count() * 8;
+  launch(k_schedulefree, (unsigned)(tiles < gmax ? tiles : gmax), 256, 0, st, (const Seg*)d_segs, n_seg, tiles, scalars_dev,
+         (float)weight_decay, weight_decay != 0.0 ? 1 : 0, first_step ? 1 : 0);
+  TP_LAUNCH_CHECK();
+  return TP_OK;
+}
+
+int tp_schedulefree_swap(void* const* y, const void* const* z, const int64_t* numel, int n_seg, double weight,
+                         int table_cached, void* ws, size_t ws_bytes, void* stream) {
+  if (!numel || n_seg <= 0 || !ws) return TP_ERR_INVALID;
+  if (!table_cached && (!y || !z)) return TP_ERR_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  Arena ar(ws, ws_bytes);
+  Seg* d_segs = nullptr; long long tiles = 0;
+  int rc = seg_table(ar, table_cached, y, nullptr, (void* const*)z, numel, n_seg, &d_segs, &tiles, st);
+  if (rc) return rc;
+  if (tiles == 0) return TP_OK;
+  const long long gmax = (long long)sm_count() * 8;
+  launch(k_lerp_segs, (unsigned)(tiles < gmax ? tiles : gmax), 256, 0, st, (const Seg*)d_segs, n_seg, tiles, (float)weight);
   TP_LAUNCH_CHECK();
   return TP_OK;
 }

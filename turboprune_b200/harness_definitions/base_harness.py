@@ -9,7 +9,10 @@ Same attributes and methods the driver relies on (``.model .train_loader .val_lo
     of the whole step (replayed from the third step of a level on);
   * the per-step ``loss.item()`` host sync (reference :134) is deferred: losses accumulate on the device and are
     read once per epoch;
-  * accuracy is a two-integer device counter instead of torchmetrics (not installed).
+  * accuracy is a two-integer device counter instead of torchmetrics (not installed);
+  * a schedule-free optimizer (one with ``train()`` / ``eval()``) is put in train mode by ``train_step`` and in eval
+    mode by ``test()``, so evaluation and the checkpoints saved after it see the averaged weights x (the reference never
+    calls either, so its evaluation and checkpoints see the training iterate y).
 """
 from contextlib import nullcontext
 
@@ -163,6 +166,7 @@ class BaseHarness:
         inputs, targets = inputs.to(self.device, non_blocking=True), targets.to(self.device, non_blocking=True)
         if not inputs.is_cuda:
             raise RuntimeError("turboprune_b200: the train step needs CUDA tensors (H100 / sm_90a); there is no CPU path")
+        self._optimizer_mode(train=True)  # in place: a captured step stays valid across the switches
         sync_lr = getattr(self.optimizer, "sync_lr", None)
         key = self._graph_key(inputs, targets)
         g = self._graph if self._graph_enabled() else None
@@ -212,6 +216,14 @@ class BaseHarness:
         self._drop_staged()
         return {"loss": loss}
 
+    def _optimizer_mode(self, train: bool):
+        """Schedule-free optimizers keep the weights at y to train and at the average x to evaluate; ``train()`` /
+        ``eval()`` move them (no-ops when already there).  Other optimizers have neither method."""
+        opt = getattr(self, "optimizer", None)
+        fn = getattr(opt, "train" if train else "eval", None)
+        if callable(fn) and callable(getattr(opt, "eval" if train else "train", None)):
+            fn()
+
     def _drop_staged(self):
         """A staged operand pair must never outlive its step (a layer skipped by this forward would otherwise feed the
         next eval / pruning forward bf16 weights from before optimizer.step())."""
@@ -251,6 +263,7 @@ class BaseHarness:
 
     def test(self):
         self.model.eval()
+        self._optimizer_mode(train=False)
         if self.distributed:        # the reference's DDP broadcasts rank 0's BN statistics on every forward
             for m in self.model.modules():
                 if isinstance(m, nn.modules.batchnorm._BatchNorm) and m.running_mean is not None:

@@ -5,8 +5,9 @@ reference's behaviour (:28-50, :159-269): a fresh optimizer and LR schedule per 
 over), ``model_init.pt`` / ``optimizer_init.pt`` at level 0, ``model_rewind.pt`` at ``pruning_params.rewind_epoch``,
 per-level CSV + summary CSV.  Optimizer = ``FusedSGD`` (same state-dict layout as torch.optim.SGD), or ``FusedAdamW``
 (torch.optim.AdamW's) when ``optimizer_params.optimizer_name`` is ``AdamW``, or ``FusedMuon`` (Muon for the hidden masked
-weights, AdamW for the rest) when it is ``MuonAdamW``.  Loaders: the
-reference's device-resident CIFAR loader (``AirbenchLoaders``) when a CIFAR config names a ``dataset_params.dataloader_type``
+weights, AdamW for the rest) when it is ``MuonAdamW``, or ``FusedScheduleFreeSGD`` with no LR scheduler whatever the name
+says when ``optimizer_params.scheduler_type`` is ``ScheduleFree`` (the reference's ``schedulefree.SGDScheduleFree``).
+Loaders: the reference's device-resident CIFAR loader (``AirbenchLoaders``) when a CIFAR config names a ``dataset_params.dataloader_type``
 other than ``synthetic`` (the reference's ``dp_cifar*.yaml`` say ``torch``); ``ImageFolderImagenet`` (GPU-decoded
 ImageFolder tree) when an ImageNet config says ``dataloader_type: imagefolder``; otherwise (FFCV / WebDataset are out of
 scope) the synthetic on-device generator.
@@ -25,7 +26,7 @@ import torch
 import torch.nn as nn
 from torch.amp import autocast
 
-from ..optim import FusedAdamW, FusedMuon, FusedSGD
+from ..optim import FusedAdamW, FusedMuon, FusedScheduleFreeSGD, FusedSGD
 from ..utils import schedulers
 from ..utils.custom_models import CustomModel, TorchVisionModel
 from ..utils.dataset import AirbenchLoaders, ImageFolderImagenet, SyntheticLoaders
@@ -75,10 +76,17 @@ class PruningHarness(BaseHarness):
 
     def _setup_optimizer(self):
         o = self.cfg.optimizer_params
-        if o.scheduler_type == "ScheduleFree":
-            raise NotImplementedError("ScheduleFree optimizer (third-party package, off the benchmarked path)")
         # capturable: the learning rate is a device scalar refreshed by train_step (sync_lr), so the captured step
         # follows the per-iteration LR schedule without being re-recorded
+        if o.scheduler_type == "ScheduleFree":
+            # the reference builds schedulefree.SGDScheduleFree for this scheduler whatever optimizer_name says
+            if o.get("warmup_steps") is None:
+                raise ValueError("scheduler_type ScheduleFree needs optimizer_params.warmup_steps (the number of "
+                                 "linear warm-up steps of the schedule-free learning rate)")
+            self.optimizer = FusedScheduleFreeSGD(self.model.parameters(), lr=o.lr, momentum=o.momentum,
+                                                  weight_decay=o.weight_decay, warmup_steps=o.warmup_steps,
+                                                  capturable=True)
+            return
         if o.get("optimizer_name", "SGD") == "AdamW":
             self.optimizer = FusedAdamW(self.model.parameters(), lr=o.lr, betas=tuple(o.get("betas") or (0.9, 0.999)),
                                         eps=o.get("eps") or 1e-8, weight_decay=o.weight_decay, capturable=True)
@@ -115,7 +123,9 @@ class PruningHarness(BaseHarness):
 
     def _setup_scheduler(self, epochs_per_level):
         kind = self.cfg.optimizer_params.scheduler_type
-        if kind == "OneCycleLR":
+        if kind == "ScheduleFree":
+            self.scheduler = None                  # the schedule is the optimizer's own
+        elif kind == "OneCycleLR":
             self.scheduler = torch.optim.lr_scheduler.OneCycleLR(self.optimizer, max_lr=self.cfg.optimizer_params.lr,
                                                                  epochs=epochs_per_level, steps_per_epoch=len(self.train_loader))
         elif kind == "TriangularSchedule":
@@ -197,6 +207,7 @@ class PruningHarness(BaseHarness):
         from ..utils.pruning_utils import rigl_update
         inputs, targets = batch
         inputs, targets = inputs.to(self.device, non_blocking=True), targets.to(self.device, non_blocking=True)
+        self._optimizer_mode(train=True)           # a schedule-free optimizer scores and regrows at y
         store = self._grad_store()
         store.zero()
         with self._compute_precision(), ops.dense_weight_grad():

@@ -458,6 +458,35 @@ def adamw_step(params, grads, exp_avgs, exp_avg_sqs, steps, inv_lr_dev, decay_de
     _count(2)
 
 
+def schedulefree_step(params, grads, zs, scalars_dev, weight_decay, first_step, table_ws=None, table_cached=False):
+    """One fused Schedule-Free SGD step (one launch).  ``scalars_dev``: device fp32 [3] = (lr, ckp1, alpha_y), each
+    formed in double.  ``first_step``: the ``zs`` are uninitialised and start as copies of the params.  ``table_ws`` /
+    ``table_cached``: as ``sgd_momentum_step``."""
+    lib = _cabi.load()
+    dev = params[0].device
+    wsb = table_ws if table_ws is not None else _workspace(lib.tp_segtable_workspace_bytes(len(params)), dev, "seg")
+    ptrs = [None] * 3 if table_cached else [_cabi.ptr_array(ts) for ts in (params, grads, zs)]
+    with torch.cuda.device(dev):
+        rc = lib.tp_schedulefree_sgd(*ptrs, _cabi.i64_array([p.numel() for p in params]), len(params),
+                                     c_void_p(scalars_dev.data_ptr()), float(weight_decay), int(bool(first_step)),
+                                     int(bool(table_cached)), c_void_p(wsb.data_ptr()), wsb.numel(), _cabi.stream_ptr(dev))
+    _cabi.check(rc, "tp_schedulefree_sgd")
+    _count()
+
+
+def schedulefree_swap(params, zs, weight, table_ws=None, table_cached=False):
+    """``p.lerp_(z, weight)`` for every pair, bit for bit with torch's per-tensor lerp_, in one launch."""
+    lib = _cabi.load()
+    dev = params[0].device
+    wsb = table_ws if table_ws is not None else _workspace(lib.tp_segtable_workspace_bytes(len(params)), dev, "seg")
+    ptrs = [None] * 2 if table_cached else [_cabi.ptr_array(ts) for ts in (params, zs)]
+    with torch.cuda.device(dev):
+        rc = lib.tp_schedulefree_swap(*ptrs, _cabi.i64_array([p.numel() for p in params]), len(params), float(weight),
+                                      int(bool(table_cached)), c_void_p(wsb.data_ptr()), wsb.numel(), _cabi.stream_ptr(dev))
+    _cabi.check(rc, "tp_schedulefree_swap")
+    _count()
+
+
 MUON_GRAM, MUON_POLY, MUON_UPDATE = 0, 1, 2
 
 

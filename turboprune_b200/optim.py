@@ -1,5 +1,5 @@
-"""Fused SGD(momentum, weight_decay) — one kernel launch for all parameters — fused AdamW (``FusedAdamW``) and fused
-Muon with AdamW for the remaining parameters (``FusedMuon``).
+"""Fused SGD(momentum, weight_decay) — one kernel launch for all parameters — fused AdamW (``FusedAdamW``), fused
+Muon with AdamW for the remaining parameters (``FusedMuon``) and fused Schedule-Free SGD (``FusedScheduleFreeSGD``).
 
 Same update rule and state layout as ``torch.optim.SGD`` as the reference configures it
 (harness_definitions/standard_pruning_harness.py:70-75): ``g += wd*w; buf = mu*buf + g
@@ -199,6 +199,153 @@ class FusedAdamW(_AdamWGroups, torch.optim.Optimizer):
             if ps:
                 self._launch(gi, group, ps)
         return loss
+
+
+def _schedulefree_advance(group):
+    """One step of a Schedule-Free group's host schedule, in Python floats as the schedulefree package writes it: commits
+    ``k + 1``, ``lr_max``, ``weight_sum`` and ``scheduled_lr`` and returns the step's (lr, ckp1, alpha_y)."""
+    k, warmup = group["k"], group["warmup_steps"]
+    sched = (k + 1) / warmup if k < warmup else 1.0
+    lr = group["lr"] * sched
+    lr_max = group["lr_max"] = max(lr, group["lr_max"])
+    weight = ((k + 1) ** group["r"]) * (lr_max ** group["weight_lr_power"])
+    weight_sum = group["weight_sum"] = group["weight_sum"] + weight
+    ckp1 = weight / weight_sum if weight_sum != 0 else 0
+    group["scheduled_lr"] = lr
+    group["k"] = k + 1
+    return lr, ckp1, lr * (group["momentum"] * (1 - ckp1) - 1)
+
+
+class FusedScheduleFreeSGD(torch.optim.Optimizer):
+    """Schedule-Free SGD (Defazio et al. 2024, "The Road Less Scheduled"): the schedulefree package's ``SGDScheduleFree``
+    with one fused launch per parameter group (``tp_schedulefree_sgd``, 20 B/elem), bit for bit with the package's
+    foreach torch ops on the same GPU.  Group keys (``lr, momentum, weight_decay, warmup_steps, r, weight_lr_power, k,
+    weight_sum, lr_max, scheduled_lr, train_mode, foreach``) and the per-parameter state ``z`` are the package's, so
+    ``state_dict()`` keeps its layout.
+
+    The parameters hold y while training and the average x = lerp(y, z, 1 - 1 / momentum) otherwise.  ``eval()`` moves
+    them to x and ``train()`` back to y (``tp_schedulefree_swap``: one launch, eager, no host sync); each is a no-op when
+    the optimizer is already in that mode, and ``step()`` raises outside train mode.  The optimizer starts in eval mode:
+    call ``train()`` before training and ``eval()`` before evaluating or saving (the harness does both).
+
+    The schedule (``k`` and the values formed from it) advances exactly once per update:
+      * ``capturable=False``: ``step()`` advances it, fills the step's device scalars and launches;
+      * ``capturable=True``: ``sync_lr()`` advances it and fills the device scalars (``fill_``, no host sync); ``step()``
+        only launches, so it may run eagerly, be captured into a CUDA graph, or both, after one ``sync_lr()``, and a
+        replay needs ``sync_lr()`` first.  Call ``sync_lr()`` once before every update.
+    A parameter whose first gradient arrives late gets its ``z`` in a launch of its own.  The package also adds the
+    weight decay into ``p.grad``; this optimizer leaves the gradient as it is.  Closures are not supported."""
+
+    def __init__(self, params, lr=1.0, momentum=0.9, weight_decay=0, warmup_steps=0, r=0.0, weight_lr_power=2.0, *,
+                 capturable=False):
+        for name, v in (("lr", lr), ("momentum", momentum), ("weight_decay", weight_decay), ("warmup_steps", warmup_steps),
+                        ("r", r), ("weight_lr_power", weight_lr_power)):
+            if isinstance(v, torch.Tensor):
+                raise ValueError(f"FusedScheduleFreeSGD: {name} must be a Python number (the device scalars are its own)")
+        if not 0.0 <= lr:
+            raise ValueError(f"Invalid learning rate: {lr}")
+        if not 0.0 <= weight_decay:
+            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
+        if not 0.0 < momentum < 1.0:
+            raise ValueError(f"Momentum must be between 0 and 1 exclusive: {momentum}")
+        defaults = dict(lr=lr, momentum=momentum, r=r, k=0, warmup_steps=warmup_steps, train_mode=False,
+                        weight_sum=0.0, lr_max=-1.0, scheduled_lr=0.0, weight_lr_power=weight_lr_power,
+                        weight_decay=weight_decay, foreach=True)
+        super().__init__(params, defaults)
+        for group in self.param_groups:
+            for p in group["params"]:
+                if torch.is_complex(p) or p.dtype != torch.float32:
+                    raise ValueError(f"FusedScheduleFreeSGD: fp32 parameters only, not {p.dtype}")
+        self.capturable = capturable
+        self._host = {}           # group -> the step's (lr, ckp1, alpha_y) as Python floats
+        self._sc_dev = {}         # (group, device) -> fp32 [lr, ckp1, alpha_y]
+        self._table = {}          # (group, device) / (group, device, "swap") -> (pointer signature, workspace)
+
+    def _fill(self, gi, t):
+        # three fill_ launches, no host-to-device copy; fill_ rounds each double to fp32 as Scalar.to<float>() does
+        for i, v in enumerate(self._host[gi]):
+            t[i].fill_(v)
+
+    def sync_lr(self):
+        """Capturable: advance every group's schedule by one update and refresh its device scalars (call once before
+        every update, eager or replayed).  Without ``capturable`` ``step()`` does this and this call does nothing."""
+        if not self.capturable:
+            return
+        for gi, group in enumerate(self.param_groups):
+            self._host[gi] = _schedulefree_advance(group)
+        for (gi, _), t in self._sc_dev.items():
+            self._fill(gi, t)
+
+    @torch.no_grad()
+    def train(self):
+        """Move every parameter with a ``z`` from x to y (lerp weight 1 - momentum) and enter train mode."""
+        self._swap(True)
+
+    @torch.no_grad()
+    def eval(self):
+        """Move every parameter with a ``z`` from y to x (lerp weight 1 - 1 / momentum) and enter eval mode."""
+        self._swap(False)
+
+    def _swap(self, to_train):
+        for gi, group in enumerate(self.param_groups):
+            if group["train_mode"] == to_train:
+                continue
+            ps = [p for p in group["params"] if "z" in self.state[p]]
+            if ps:
+                momentum = group["momentum"]
+                zs = [self.state[p]["z"] for p in ps]
+                ws, hit = self._workspace((gi, ps[0].device, "swap"), ps, zs)
+                ops.schedulefree_swap(ps, zs, 1 - momentum if to_train else 1 - 1 / momentum, table_ws=ws, table_cached=hit)
+            group["train_mode"] = to_train
+
+    def _workspace(self, key, *lists):
+        sig = tuple(t.data_ptr() for ts in lists for t in ts)
+        nbytes = _cabi.load().tp_segtable_workspace_bytes(len(lists[0]))
+        cached = self._table.get(key)
+        if cached is None or cached[1].numel() < nbytes:
+            cached = (None, torch.empty(nbytes, dtype=torch.uint8, device=lists[0][0].device))
+        self._table[key] = (sig, cached[1])
+        return cached[1], cached[0] == sig
+
+    @torch.no_grad()
+    def step(self, closure=None):
+        if closure is not None:
+            raise NotImplementedError("FusedScheduleFreeSGD.step does not take a closure")
+        if not self.param_groups[0]["train_mode"]:
+            raise RuntimeError("FusedScheduleFreeSGD: step() outside train mode: call optimizer.train() before training "
+                               "and optimizer.eval() before evaluating or saving")
+        for gi, group in enumerate(self.param_groups):
+            if not self.capturable:
+                self._host[gi] = _schedulefree_advance(group)
+            elif gi not in self._host:
+                raise RuntimeError("FusedScheduleFreeSGD(capturable=True): call sync_lr() before every update")
+            ps = [p for p in group["params"] if p.grad is not None]
+            old = [p for p in ps if "z" in self.state[p]]
+            new = [p for p in ps if "z" not in self.state[p]]
+            if old:
+                self._launch(gi, group, old, False)
+            if new:
+                self._launch(gi, group, new, True)
+
+    def _launch(self, gi, group, ps, first):
+        dev = ps[0].device
+        sc = self._sc_dev.get((gi, dev))
+        if sc is None:
+            sc = self._sc_dev[(gi, dev)] = torch.empty(3, dtype=torch.float32, device=dev)
+            self._fill(gi, sc)
+        elif not self.capturable:
+            self._fill(gi, sc)
+        for p in ps:
+            if p.grad.is_sparse:
+                raise RuntimeError("FusedScheduleFreeSGD does not support sparse gradients")
+            if not p.is_contiguous():
+                raise TypeError("FusedScheduleFreeSGD: contiguous fp32 parameters")
+            if first:
+                self.state[p]["z"] = torch.empty_like(p, memory_format=torch.contiguous_format)
+        grads = [p.grad if p.grad.is_contiguous() else p.grad.contiguous() for p in ps]
+        zs = [self.state[p]["z"] for p in ps]
+        ws, hit = self._workspace((gi, dev), ps, grads, zs)
+        ops.schedulefree_step(ps, grads, zs, sc, group["weight_decay"], first, table_ws=ws, table_cached=hit)
 
 
 MUON_NS_COEFFICIENTS = (3.4445, -4.7750, 2.0315)      # torch.optim.Muon's defaults (Keller Jordan's quintic)

@@ -248,8 +248,8 @@ def rigl_update(model: nn.Module, optimizer, k_per_layer, new_masks=None):
     sync_masks_from_rank0_(new_masks)
     state = getattr(optimizer, "state", {}) if optimizer is not None else {}
     per_layer = [state[m.weight] if m.weight in state else {} for m in layers]
-    # every per-element state the optimizer keeps (SGD: momentum_buffer; AdamW: exp_avg, exp_avg_sq; AdamW's
-    # per-parameter step is left alone); SGD, or no state at all, keeps the one-state apply
+    # every per-element state the optimizer keeps (SGD: momentum_buffer; AdamW: exp_avg, exp_avg_sq; Schedule-Free: z;
+    # AdamW's per-parameter step is left alone); one state, or none at all, keeps the one-state apply
     keys = [k for k in _RIGL_RESTART_KEYS if any(k in st for st in per_layer)] or ["momentum_buffer"]
     states = [[st.get(k) for st in per_layer] for k in keys]
     if len(keys) == 1:
@@ -259,7 +259,7 @@ def rigl_update(model: nn.Module, optimizer, k_per_layer, new_masks=None):
     return counts
 
 
-_RIGL_RESTART_KEYS = ("momentum_buffer", "exp_avg", "exp_avg_sq")
+_RIGL_RESTART_KEYS = ("momentum_buffer", "exp_avg", "exp_avg_sq", "z")
 
 
 def prune_the_model(cfg, harness, target_density: float) -> None:
